@@ -1,4 +1,4 @@
-"""bench.py — TransFuser training-step throughput (samples/s of RGB+LiDAR pairs) on N B200s of one node.
+"""bench.py — TransFuser training-step throughput (samples/s of RGB+LiDAR pairs) on N H100s of one node.
 
   python bench.py --gpus 1 --steps 20 --warmup 3          # this repo's CUDA path (default)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
@@ -6,7 +6,11 @@
 
 One "step" = BASELINE.json configs[1]: LidarCenterNet (TransFuser, RegNetY-3.2GF) forward + backward + AdamW on a batch of
 10 samples per GPU (160x704 RGB + 40k LiDAR points -> 2x256x256 BEV histogram on the GPU + target-point image), dropout on,
-all 11 losses, synthetic data, random-init weights. Prints ONE JSON line (rank 0)."""
+all 11 losses, synthetic data, random-init weights. Prints ONE JSON line (rank 0).
+
+  python bench.py ... --dump-outputs DIR                  # also write what the last timed step computed to DIR/<name>.npy
+
+Inputs and initial weights are seeded, so two builds run with the same arguments can be compared output for output."""
 import argparse
 import json
 import math
@@ -27,10 +31,20 @@ METRIC = 'training samples/sec (RGB+LiDAR pairs)'
 
 
 def peaks():
+    """Roofline peaks: H100 SXM data sheet (700 W card; dense BF16), never reached figures."""
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0), 'H100 SXM data sheet'
+
+
+def gpu_identity(index=0):
+    """Card name and power limit, read in the same run as the measurement they qualify."""
     try:
-        return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))), 'measured'
-    except Exception:
-        return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0), 'fallback'
+        r = subprocess.run(['nvidia-smi', '-i', str(index), '--query-gpu=name,power.limit', '--format=csv,noheader,nounits'],
+                           capture_output=True, text=True, timeout=30)
+        name, limit = [c.strip() for c in r.stdout.strip().split(',')[:2]]
+        return {'name': name, 'power_limit_w': float(limit)}
+    except Exception:  # noqa: BLE001
+        import torch
+        return {'name': torch.cuda.get_device_name(index), 'power_limit_w': None}
 
 
 class ClockSampler:
@@ -55,6 +69,7 @@ class ClockSampler:
         if self.proc is None:
             return dict(sm_mhz=None, sm_max_mhz=None, reasons=['nvidia-smi unavailable'])
         self.proc.terminate()
+        self.proc.wait()
         sm = sorted(float(r[0]) for r in self.rows if r and r[0].replace('.', '').isdigit())
         reasons = set()
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
@@ -133,6 +148,7 @@ def run_b200(args):
         torch.cuda.synchronize()
 
     resident = [None]
+    last_loss = [None]               # the total-loss tensor of the latest timed step
 
     def timed(n, e2e):
         resident[0] = h2d()
@@ -142,7 +158,7 @@ def run_b200(args):
         e0.record()
         last = None
         for _ in range(n):
-            loss = run_step(e2e)
+            loss = last_loss[0] = run_step(e2e)
             if e2e:
                 last = float(loss.item())  # device -> host read of the step's result
         e1.record()
@@ -165,8 +181,10 @@ def run_b200(args):
     if rank == 0:
         sampler.start()
     ms_dev, launches, _ = timed(args.steps, e2e=False)
-    ms_e2e, _, last_loss = timed(args.steps, e2e=True)
+    ms_e2e, _, e2e_loss = timed(args.steps, e2e=True)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, tr, last_loss[0], torch, np)
 
     # ---- roofline of the dominant kernel: per-entry-point CUDA-event timing over one extra step (rank 0) ----
     roof = None
@@ -192,11 +210,6 @@ def run_b200(args):
         except Exception as e:  # noqa: BLE001 — the eager-event figures stay in the line; say why the graph timing is missing
             roof['graph_timing_error'] = repr(e)[:200]
         prof.calls = None
-        if os.path.isdir(os.path.join(ROOT, 'gpurun_out')):
-            det = sorted(prof.detail.items(), key=lambda kv: -kv[1][0])
-            with open(os.path.join(ROOT, 'gpurun_out', 'profile_detail_%s.txt' % args.gemm), 'w') as f:
-                for k, (ms, n, fl) in det:
-                    f.write('%9.3f ms  x%-4d %7.2f TF/s  %s\n' % (ms, n, (fl * n / (ms * 1e-3) / 1e12) if ms > 0 else 0.0, k))
     h2d_bytes = sum(v.numel() * v.element_size() for v in host.values())
     if rank == 0:
         pk, how = peaks()
@@ -214,10 +227,10 @@ def run_b200(args):
                        'global_batch': total, 'parallelism': 'dp%d' % world, 'gemm_mode': args.gemm,
                        'inputs': ('raw (uint8 frames, points, pose transform, target point): model inputs built by the GPU input pipeline inside the step'
                                   if raw else 'expanded fp32 / int64 tensors as the reference DataLoader ships them; LiDAR points -> BEV histogram on the GPU'), 'cuda_graph': tr.graph is not None, 'cuda_graph_error': tr.graph_error,
-                       'l2': 'working set (672 MB weights + activations) exceeds the 126 MB L2; no explicit flush'},
+                       'l2': 'working set (672 MB weights + activations) exceeds the 50 MB L2; no explicit flush'},
             'e2e': {'value': round(e2e_v, 3), 'unit': 'samples/s', 'ms_per_step': round(ms_e2e / args.steps, 3),
-                    'h2d_bytes_per_step': h2d_bytes, 'd2h_bytes_per_step': 4, 'last_loss': last_loss},
-            'gpu_launches': launches, 'clocks': clocks,
+                    'h2d_bytes_per_step': h2d_bytes, 'd2h_bytes_per_step': 4, 'last_loss': e2e_loss},
+            'gpu': gpu_identity(local), 'gpu_launches': launches, 'clocks': clocks,
             'step_tensor_roofline': {'achieved_tflops': round(flop_per_sample * value / 1e12, 2), 'peak_tflops': pk['bf16_tflops_sustained'],
                                      'frac': round(flop_per_sample * value / 1e12 / pk['bf16_tflops_sustained'], 4), 'of': how},
             'roofline': roof,
@@ -238,7 +251,7 @@ def graph_timed_roofline(prof, torch, _lib, replays=5):
     dedicated CUDA graph and timed with CUDA events: per-launch device time without the host launch path that eager per-call events
     include. achieved = algorithmic FLOPs (or bytes) of those launches / that time. `roof_frac` compares with the BINDING roofline
     of each launch — max(FLOPs / tensor peak, algorithmic bytes / HBM peak) — because the same kernel serves tensor-bound GPT GEMMs
-    and HBM-bound 72..576-channel 1x1 convs. `traffic`: measured DRAM bytes per launch from the committed ncu capture, if present."""
+    and HBM-bound 72..576-channel 1x1 convs."""
     pk, how = peaks()
     names = set(prof.top_entry_points)
     calls = [(n, a) for n, a in prof.calls if n in names]
@@ -293,23 +306,23 @@ def graph_timed_roofline(prof, torch, _lib, replays=5):
         achb = sum(w[0] for _, _, w in big) / (msb * 1e-3) / 1e12
         out['large_launches'] = {'what': 'launches with >= 10 GFLOP (the C = 1512 GPT GEMMs)', 'launches': len(big), 'ms_per_step': round(msb, 3),
                                  'achieved': round(achb, 2), 'unit': 'TFLOP/s', 'frac': round(achb / pk['bf16_tflops_sustained'], 4)}
-    try:
-        tr = json.load(open(os.path.join(ROOT, 'profiles', 'r2_ncu_traffic.json')))
-        ent = tr.get(roof_kernel_key(prof))
-        if ent:
-            out['traffic'] = ent['dram_bytes_per_launch']
-            out['traffic_source'] = ent['source']
-            out['algorithmic_bytes_per_launch'] = round(by / len(calls))
-    except Exception:
-        pass
     return out
 
 
-def roof_kernel_key(prof):
-    for k, v in prof.families.items():
-        if v[4] == prof.top_entry_points:
-            return k
-    return None
+def dump_outputs(out_dir, tr, loss, torch, np, n_sample=1 << 20):
+    """Writes what the last timed step computed, as a caller of Trainer.step receives it: the weighted total loss, the 11 loss
+    terms, and the parameters and gradients the step left in the flat buffers (the same seeded sample of n_sample elements of
+    each; 8 MB in all). float64 for the losses, float32 for the rest."""
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, 'loss_total.npy'), np.array([float(loss.detach())], dtype=np.float64))
+    for k, v in tr.last_losses.items():
+        np.save(os.path.join(out_dir, '%s.npy' % k), np.array([float(v)], dtype=np.float64))
+    total = tr.flat.total
+    idx = np.unique(np.random.default_rng(0).integers(0, total, size=min(n_sample, total)))
+    it = torch.from_numpy(idx).to(tr.flat.flat.device)
+    np.save(os.path.join(out_dir, 'params_sample.npy'), tr.flat.flat[it].float().cpu().numpy())
+    np.save(os.path.join(out_dir, 'grads_sample.npy'), tr.flat.grad[it].float().cpu().numpy())
 
 
 def effective_cores():
@@ -405,13 +418,14 @@ def main():
     ap.add_argument('--batch', type=int, default=0, help='samples per GPU (default: the batch of --config; configs[1]: 10)')
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference', 'cpu_baseline'])
     ap.add_argument('--gemm', default=os.environ.get('TFB_GEMM', 'bf16'), choices=['simt', 'bf16', 'bf16x3', 'bf16x6'],
-                    help="bf16: tcgen05 bf16 operands (the benched mode); bf16x6 / bf16x3: the tensor-core parity modes (fp32 operands as three / two bf16 terms, six / three "
-                         "tcgen05 products per fp32 product); simt: exact fp32 on the CUDA cores")
+                    help="bf16: wgmma bf16 operands (the benched mode); bf16x6 / bf16x3: the tensor-core parity modes (fp32 operands as three / two bf16 terms, six / three "
+                         "wgmma products per fp32 product); simt: exact fp32 on the CUDA cores")
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--raw-inputs', type=int, default=int(os.environ.get('TFB_RAW_INPUTS', '1')),
                     help='1: feed the step with what is on disk (uint8 frames, raw points, pose transform; 1.6 MB per sample over PCIe) and '
                          'build the model inputs on the GPU inside the step; 0: the expanded fp32 / int64 tensors of the reference DataLoader (3.8 MB)')
     ap.add_argument('--graph', type=int, default=1, help='1: capture the whole step (incl. the NCCL gradient all-reduce when N > 1) in a CUDA graph; 0: eager')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR', help='write the losses, parameters and gradients of the last timed step to DIR/<name>.npy')
     args = ap.parse_args()
     if args.impl == 'cpu_baseline':
         print(json.dumps(cpu_reference(steps=2, warmup=0, batch=1, budget_s=120.0)), flush=True)

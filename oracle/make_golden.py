@@ -1,5 +1,5 @@
 """ORACLE / TEST INFRASTRUCTURE ONLY. Generates the committed fixtures under tests/golden/ by executing the REFERENCE
-itself (imported verbatim from /root/reference via oracle/ref_import.py) on seeded inputs. Run in the build container:
+itself (imported verbatim from a reference checkout via oracle/ref_import.py) on seeded inputs. Run in the build container:
     python oracle/make_golden.py [bev] [model] [pipeline]
 """
 import os

@@ -1,7 +1,7 @@
 """ORACLE / TEST INFRASTRUCTURE ONLY — never imported by the product path.
 
 numpy restatement of the per-sample input preparation of the reference's dataset class (CARLA_Data.__getitem__,
-/root/reference/team_code_transfuser/data.py:103-356) for the pieces SURVEY.md §8f rank 2 moves to the GPU:
+team_code_transfuser/data.py:103-356) for the pieces SURVEY.md §8f rank 2 moves to the GPU:
   align                 data.py:411-443   (+ utils.py:14-27 transforms)
   draw_target_point     data.py:616-630   (cv2.circle radius 5 thickness 3: restated as a 15x15 stamp, see STAMP below)
   crop_image_cv2        data.py:536-551,  crop_seg data.py:561-576, get_depth data.py:358-372, converter LUT data.py:235

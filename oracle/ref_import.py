@@ -1,7 +1,7 @@
 """ORACLE / TEST INFRASTRUCTURE ONLY — never imported by the product path.
 
-Imports the reference's own modules VERBATIM from /root/reference (read-only, this container
-only — the GPU box has no /root/reference) behind the shim packages in oracle/shims for the
+Imports the reference's own modules VERBATIM from a checkout of autonomousvision/transfuser (branch 2022) — the directory
+named by $TRANSFUSER_REFERENCE, by default `reference/` next to this repository — behind the shim packages in oracle/shims for the
 un-vendored dependencies (timm, mmcv, mmdet, torch_scatter).  Used to (1) validate the CPU
 restatement in oracle/torch_oracle.py and (2) generate the committed fixtures in tests/golden/
 (oracle/make_golden.py).
@@ -10,7 +10,8 @@ import importlib
 import os
 import sys
 
-REF_ROOT = '/root/reference/team_code_transfuser'
+REF_ROOT = os.path.join(os.environ.get('TRANSFUSER_REFERENCE', os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), 'reference')),
+                        'team_code_transfuser')
 SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'shims')
 
 

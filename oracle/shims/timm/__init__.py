@@ -1,7 +1,7 @@
 """ORACLE / TEST INFRASTRUCTURE ONLY — never imported by the product path.
 
 Stand-in for the un-vendored dependency `timm==0.5.4`
-(/root/reference/team_code_transfuser/requirements.txt:104), restating from its
+(team_code_transfuser/requirements.txt:104), restating from its
 published definition the single model the hot path constructs:
 `timm.create_model('regnety_032', ...)` (call sites transfuser.py:380,442).
 

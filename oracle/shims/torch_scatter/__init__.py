@@ -1,4 +1,4 @@
-"""ORACLE / TEST INFRASTRUCTURE ONLY. Empty stand-in so /root/reference/team_code_transfuser/point_pillar.py:6
+"""ORACLE / TEST INFRASTRUCTURE ONLY. Empty stand-in so team_code_transfuser/point_pillar.py:6
 imports; PointPillars is off by default (config.py:42) and out of scope."""
 
 

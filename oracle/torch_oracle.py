@@ -2,7 +2,7 @@
 bench.py's cpu_baseline / --impl reference legs may use it, and only as the checker / the CPU arm).
 
 CPU restatement, in stock fp32 PyTorch functional ops, of the reference's training hot path:
-  LidarCenterNet.forward            /root/reference/team_code_transfuser/model.py:733-805
+  LidarCenterNet.forward            team_code_transfuser/model.py:733-805
   TransfuserBackbone.forward        transfuser.py:120-211   (GPT 333-366, Block 545-549, SelfAttention 510-527)
   SegDecoder / DepthDecoder         transfuser.py:239-246, 273-281
   forward_gru                       model.py:611-646
@@ -56,7 +56,7 @@ def _q(t):
 
 
 def _tc_gemm(M, N, K):
-    """Shapes transfuser_b200.gemm.tc_ok sends to the tcgen05 GEMM (TMA: 16-byte aligned rows); the rest stays exact fp32."""
+    """Shapes transfuser_b200.gemm.tc_ok sends to the tensor-core GEMM (TMA: 16-byte aligned rows); the rest stays exact fp32."""
     return M >= 32 and N >= 16 and K >= 16 and K % 8 == 0 and N % 8 == 0
 
 

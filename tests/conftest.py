@@ -13,13 +13,13 @@ def pytest_configure(config):
     # the torch ops used as fp32 references must really be fp32 (cuDNN / cuBLAS default to TF32 for convs)
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box via gpurun)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100: sm_90a)')
 
 
 @pytest.fixture(scope='session', autouse=True)
 def _built_library():
     """The C-ABI library is a build product (git-ignored): build it once per session if it is not there yet
-    (nvcc cross-compiles sm_100a without a GPU)."""
+    (nvcc cross-compiles sm_90a without a GPU)."""
     from transfuser_b200 import build as b
     if not os.path.isfile(b.LIB):
         b.build(verbose=False)

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY. Builds tests/cuda_emul/_build/libtfb200_emul.so: the SIMT .cu files of transfuser_b200/csrc
 compiled for the host against the emulation header (see cuda_emul.h). The only source transformation is the launch syntax:
     kernel<<<grid, block, smem, stream>>>(args);   ->   emul_launch(grid, block, [=] { kernel(args); });
-The tensor-core files (gemm_tc.cu, conv_tc.cu: tcgen05 / TMA / mbarrier PTX) cannot be emulated and are left out, so their
+The tensor-core files (gemm_tc.cu, conv_tc.cu: wgmma / TMA / mbarrier PTX) cannot be emulated and are left out, so their
 entry points are absent from the emulated library."""
 import hashlib
 import os

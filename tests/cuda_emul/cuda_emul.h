@@ -49,6 +49,9 @@ typedef int cudaError_t;
 enum { cudaSuccess = 0 };
 enum { cudaDevAttrMultiProcessorCount = 16 };
 static inline cudaError_t cudaMemsetAsync(void* p, int v, size_t n, cudaStream_t) { memset(p, v, n); return cudaSuccess; }
+static inline cudaError_t cudaMalloc(void** p, size_t n) { *p = malloc(n ? n : 1); return *p ? cudaSuccess : 2; }
+enum cudaStreamCaptureMode { cudaStreamCaptureModeGlobal = 0, cudaStreamCaptureModeThreadLocal = 1, cudaStreamCaptureModeRelaxed = 2 };
+static inline cudaError_t cudaThreadExchangeStreamCaptureMode(cudaStreamCaptureMode*) { return cudaSuccess; }
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 static inline const char* cudaGetErrorString(cudaError_t) { return "emulated"; }
 static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }

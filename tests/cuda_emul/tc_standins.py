@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY. torch stand-ins for the tensor-core entry points (tcgen05 / TMA: not emulable), written from the
+"""TEST INFRASTRUCTURE ONLY. torch stand-ins for the tensor-core entry points (wgmma / TMA: not emulable), written from the
 CONTRACT in include/tfb200.h — operand layouts, leading dimensions, column windows, the packed-weight format of csrc/conv_pack.cu —
 so that the product's bf16-mode host path (sidecars, packed weights, q|k|v packs, im2col + batched wgrad, flat gradients) can run
 end to end on the CPU emulation with every CUDA-core kernel real and only the MMA itself replaced. They check what the real

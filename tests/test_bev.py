@@ -1,11 +1,12 @@
-"""BEV histogram: oracle vs the reference function / committed fixture (CPU), CUDA kernel vs oracle (GPU, bit-exact)."""
+"""BEV histogram: oracle vs the reference function's outputs / committed fixtures (CPU), CUDA kernel vs oracle (GPU, bit-exact)."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import bev_oracle, ref_import
+from oracle import bev_oracle
+from oracle.make_golden_reference import GOLD as REF_GOLD, digest
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden', 'bev_hist.npz')
 
@@ -18,15 +19,16 @@ def test_oracle_matches_golden_fixture():
         assert np.array_equal(bev_oracle.lidar_to_histogram_features(pts), g[key]), key
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_oracle_matches_reference_function():
-    ref = ref_import.load_histogram_fn()
+    """Bit-exact against the reference's lidar_to_histogram_features (data.py:446-470) on the same inputs (digests of its
+    outputs, oracle/make_golden_reference.py)."""
+    g = np.load(REF_GOLD)
     for dt in (np.float32, np.float64):
         for seed, n in ((0, 40000), (1, 1000), (2, 0), (3, 64)):
             pts = bev_oracle.synthetic_points(n, seed, dt)
             if n == 0:
                 pts = pts.reshape(0, 4)
-            assert np.array_equal(ref(pts), bev_oracle.lidar_to_histogram_features(pts))
+            assert digest(bev_oracle.lidar_to_histogram_features(pts)) == str(g['bev_%s_%d_%d' % (np.dtype(dt).name, seed, n)]), (dt, seed, n)
 
 
 @pytest.mark.gpu

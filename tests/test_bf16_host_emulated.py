@@ -1,5 +1,5 @@
 """The bf16 tensor-core mode of the product, end to end on the CPU: every CUDA-core kernel runs for real on the emulation
-(tests/cuda_emul/), only the three tcgen05 entry points are replaced by torch stand-ins written from their C-ABI contract
+(tests/cuda_emul/), only the three tensor-core entry points are replaced by torch stand-ins written from their C-ABI contract
 (tests/cuda_emul/tc_standins.py). This exercises what no other CPU test reaches — the host logic that exists only in bf16 mode:
 bf16 sidecars forward and backward, the packed-weight registry and the once-per-step batched pack, the (channel, tap) im2col feeding
 the batched wgrad GEMM that writes PyTorch-layout gradients into the flat buffer, the q|k|v pack, the bf16 weight mirror — and
@@ -16,7 +16,7 @@ TOL = 3e-2     # forward, bf16 operands (8 mantissa bits) through a few layers w
 # Gradients against the fp32 mode carry ReLU-mask flips (a bf16-perturbed pre-activation near 0 flips its mask; with the random-sign
 # upstream gradients used here one flipped element moves a column sum by ~10 %), so that comparison only has to separate "noise" from
 # "wrong layout" (a permuted tap / channel order gives a relative error >= 1). The tight gradient check is bf16-mode against bf16-mode
-# with every host-side option of DESIGN.md 4b switched off (the configuration that passed `-m gpu` on the B200 earlier in the round).
+# with every host-side option of DESIGN.md 4b switched off (the configuration the `-m gpu` tests run).
 GRAD_TOL_VS_FP32 = 0.25
 TOL_VS_PLAIN_BF16 = 3e-3    # (the fused BatchNorm + squeeze-excite backward forms dy*gate + dpool/HW with one fma inside BatchNorm's passes: 1e-7 differences, a few flipped bf16 roundings downstream)
 FLAGS = ('SIDECARS', 'SE_FUSED_BWD', 'SE_POOL_FUSED', 'QKV_FUSED', 'BN_ADD_FUSED', 'PACK_BATCHED')   # the numerically EQUIVALENT options (BN_STATS_FUSED, CONV_S2_TC, ATTN_FUSED change roundings: they stay on in both runs)

@@ -1,5 +1,5 @@
 """The tensor-core PARITY modes ('bf16x3' / 'bf16x6', transfuser_b200/gemm.py): every fp32 operand is split into two / three bf16 terms
-and each product runs as three / six tcgen05 bf16 GEMMs (smallest terms first, fp32 accumulate). Held to the fp32 tolerance of test_ops.py — 1e-4
+and each product runs as three / six tensor-core bf16 GEMMs (smallest terms first, fp32 accumulate). Held to the fp32 tolerance of test_ops.py — 1e-4
 relative L2 per op against plain fp32 torch (north_star: 1e-3) — forward and backward, for every op the mode moves to the tensor cores:
 nn.Linear / 1x1 convs (incl. stride 2), dense 3x3 convs (im2col + GEMM: forward, dgrad with flipped weights, wgrad) and the
 attention projections. The whole-model parity test (tests/test_model.py) runs in this mode as well."""

@@ -1,5 +1,5 @@
 """tests/test_bf16x3.py on the CPU: the CUDA-core kernels (operand split, im2col, reductions) run on the emulation of their sources,
-the tcgen05 GEMM is replaced by its torch stand-in (bf16 operands, fp32 accumulate — tests/cuda_emul/tc_standins.py). Checks the
+the tensor-core GEMM is replaced by its torch stand-in (bf16 operands, fp32 accumulate — tests/cuda_emul/tc_standins.py). Checks the
 host logic of the three-term mode (operand order, transposes, the flipped dgrad weights, accumulation, gradient buffers) — the
 `-m gpu` run of test_bf16x3.py is the parity test proper. Test infrastructure only."""
 import pytest

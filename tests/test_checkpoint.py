@@ -2,11 +2,11 @@
 (train.py:179-183, 381-384; submission_agent.py:92-96) load into, and are produced by, the product classes. CPU only."""
 import io
 
+import numpy as np
 import pytest
 import torch
 from torch import nn
 
-from oracle import ref_import
 from oracle import torch_oracle as O
 from transfuser_b200 import checkpoint, optim
 
@@ -101,31 +101,30 @@ def test_model_checkpoint_prefix_aliases_and_flat_views():
     assert all(k.startswith('module.') for k in torch.load(buf))
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_reference_ddp_checkpoint_loads_strict_into_product_model():
-    """A state dict written by the verbatim reference module (with the DDP prefix, as models_2022.zip's files have) loads
-    strict=True into the product module, and the agent's own loading code (k[7:], strict=False) accepts what we save."""
-    m = ref_import.load()
-    cfg = m['config'].GlobalConfig(setting='eval')
-    cfg.use_target_point_image = True
-    cfg.n_layer = 4
-    ref = m['model'].LidarCenterNet(cfg, 'cpu', 'transFuser', 'regnety_032', 'regnety_032', use_velocity=False)
-    names = [(n, tuple(p.shape)) for n, p in list(ref.named_parameters()) + list(ref.named_buffers())]
-    ref.load_state_dict(O.deterministic_state(names, seed=2), strict=False)
+    """A state dict with the verbatim reference module's keys and shapes (tests/golden/reference_checks.npz) and the DDP prefix,
+    as models_2022.zip's files have, loads strict=True into the product module, and the agent's own loading code (k[7:],
+    strict=False) finds every key it expects in what we save, and no other."""
+    from oracle.make_golden_reference import GOLD
+    g = np.load(GOLD)
+    names = [(str(n), tuple(int(d) for d in str(s).split('x') if d)) for n, s in zip(g['sd_transFuser_keys'], g['sd_transFuser_shapes'])]
     from transfuser_b200 import LidarCenterNet
     from transfuser_b200.config import TrainConfig
+    src = LidarCenterNet(TrainConfig(), 'cpu', 'transFuser', 'regnety_032', 'regnety_032', use_velocity=False)
+    own = [(n, tuple(p.shape)) for n, p in list(src.named_parameters()) + list(src.named_buffers())]
+    src.load_state_dict(O.deterministic_state(own, seed=2), strict=False)       # seeded by parameter name, aliases share the tensor
+    ref_sd = {k: src.state_dict()[k] for k, _ in names}                          # the reference's keys, in its order
     mine = LidarCenterNet(TrainConfig(), 'cpu', 'transFuser', 'regnety_032', 'regnety_032', use_velocity=False)
-    missing, unexpected = checkpoint.load_model(mine, {'module.' + k: v for k, v in ref.state_dict().items()}, strict=True)
+    missing, unexpected = checkpoint.load_model(mine, {'module.' + k: v for k, v in ref_sd.items()}, strict=True)
     assert not missing and not unexpected
-    a, b = mine.state_dict(), ref.state_dict()
-    assert all(torch.equal(a[k], b[k]) for k in b)
+    a = mine.state_dict()
+    assert all(torch.equal(a[k], v) for k, v in ref_sd.items())
     buf = io.BytesIO()
     checkpoint.save_model(mine, buf, module_prefix=True)
     buf.seek(0)
     state_dict = torch.load(buf)
     state_dict = {k[7:]: v for k, v in state_dict.items()}                  # submission_agent.py:95
-    res = ref.load_state_dict(state_dict, strict=False)
-    assert not res.missing_keys and not res.unexpected_keys
+    assert set(state_dict) == set(ref_sd) and all(tuple(state_dict[k].shape) == s for k, s in names)
 
 
 def test_parameters_without_gradient_are_left_to_the_optimizer_untouched():

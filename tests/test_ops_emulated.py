@@ -1,8 +1,8 @@
 """The per-op parity tests of tests/test_ops.py (forward and backward of every exact-fp32 kernel through the product's autograd
 wrappers, against plain fp32 torch ops) executed in this container WITHOUT a GPU: the same test functions, with the C-ABI calls
 routed to the CPU emulation of the unchanged kernel sources (tests/cuda_emul/: one OS thread per CUDA thread, barriers for
-__syncthreads / warp shuffles, launches rewritten to emul_launch). The tensor-core kernels (tcgen05 / TMA) cannot be emulated;
-everything in the exact-fp32 ("simt") numerics mode can. The `-m gpu` run of test_ops.py on a B200 remains the parity test proper:
+__syncthreads / warp shuffles, launches rewritten to emul_launch). The tensor-core kernels (wgmma / TMA) cannot be emulated;
+everything in the exact-fp32 ("simt") numerics mode can. The `-m gpu` run of test_ops.py on an H100 remains the parity test proper:
 this run checks the kernel source's indexing, control flow and arithmetic, not the device compiler. Test infrastructure only."""
 import math
 

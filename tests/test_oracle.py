@@ -1,6 +1,6 @@
-"""CPU: the oracle restatement (oracle/torch_oracle.py) against (a) the committed fixture produced by the VERBATIM
-reference and (b) — in the build container, where /root/reference exists — the reference itself; plus the structural
-cross-check of the timm shim against torchvision's RegNetY-3.2GF and the C-ABI export check."""
+"""CPU: the oracle restatement (oracle/torch_oracle.py) against the committed fixtures produced by the VERBATIM reference
+(tests/golden/model_golden.npz, tests/golden/reference_checks.npz: oracle/make_golden_model.py, oracle/make_golden_reference.py);
+plus the structural cross-check of the timm shim against torchvision's RegNetY-3.2GF and the C-ABI export check."""
 import ctypes
 import os
 
@@ -9,8 +9,26 @@ import pytest
 import torch
 
 from oracle import ref_import, torch_oracle as O
+from oracle.make_golden_reference import GOLD as REF_GOLD
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden', 'model_golden.npz')
+REF = np.load(REF_GOLD)
+
+
+def ref_names(key):
+    """(name, shape) of every state_dict entry of the reference module `key` (oracle/make_golden_reference.py MODELS), in order."""
+    return [(str(n), tuple(int(d) for d in str(s).split('x') if d)) for n, s in zip(REF['sd_%s_keys' % key], REF['sd_%s_shapes' % key])]
+
+
+def assert_same_state_dict(mine, key):
+    assert [(k, tuple(v.shape)) for k, v in mine.state_dict().items()] == ref_names(key)   # drop-in checkpoint contract
+
+
+def assert_losses(got, key, tol, floor):
+    names, want = REF['loss_%s_names' % key], REF['loss_%s' % key]
+    assert [str(n) for n in names] == list(got.keys())
+    for k, w in zip(names, want):
+        assert abs(float(w) - float(got[str(k)])) <= tol * max(abs(float(w)), floor), (key, str(k), float(w), float(got[str(k)]))
 
 
 def _product_container():
@@ -42,26 +60,19 @@ def test_oracle_reproduces_reference_golden():
     assert np.allclose(P['_model.image_encoder.features.stem.bn.running_mean'].detach().numpy(), g['stem_running_mean'], rtol=1e-5, atol=1e-6)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_oracle_and_state_dict_match_verbatim_reference():
-    from oracle.make_golden_model import reference_model
-    ref, cfg = reference_model()
+    from oracle.make_golden_model import WEIGHT_SEED
     mine = _product_container()
-    a, b = mine.state_dict(), ref.state_dict()
-    assert list(a.keys()) == list(b.keys()) and all(a[k].shape == b[k].shape for k in a)   # drop-in checkpoint contract
-    mine.load_state_dict(b, strict=True)
+    assert_same_state_dict(mine, 'transFuser')
+    P = O.deterministic_state(ref_names('transFuser'), seed=WEIGHT_SEED)
+    mine.load_state_dict(P, strict=True)
     batch = O.synthetic_batch(1, seed=2)
-    P = {k: v.clone() for k, v in ref.state_dict().items()}
 
     class C(O.Cfg):
         embd_pdrop = attn_pdrop = resid_pdrop = 0.0
     with torch.no_grad():
-        want = ref(batch['rgb'], batch['lidar'], ego_waypoint=batch['ego_waypoint'], target_point=batch['target_point'],
-                   target_point_image=batch['target_point_image'], ego_vel=batch['ego_vel'], bev=batch['bev'], label=batch['label'],
-                   depth=batch['depth'], semantic=batch['semantic'])
         got = O.forward(P, batch, C, train=True)
-    for k in want:
-        assert abs(float(want[k]) - float(got[k])) <= 1e-6 * max(abs(float(want[k])), 1e-6), k
+    assert_losses(got, 'transFuser', 1e-6, 1e-6)
 
 
 def test_timm_shim_matches_torchvision_regnet_structure():
@@ -91,73 +102,33 @@ def test_c_abi_library_exports_every_declared_symbol():
     assert cdll.tfb_abi_version() == 1
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_late_fusion_oracle_and_state_dict_match_verbatim_reference():
     """BASELINE config 5 (late_fusion.py): drop-in key set of the product module + oracle restatement vs the reference."""
-    m = ref_import.load()
-    cfg = m['config'].GlobalConfig(setting='eval')
-    cfg.use_target_point_image = True
-    torch.manual_seed(0)
-    ref = m['model'].LidarCenterNet(cfg, 'cpu', 'late_fusion', 'regnety_032', 'regnety_032', use_velocity=False).train()
     from transfuser_b200 import LidarCenterNet
     from transfuser_b200.config import TrainConfig
     mine = LidarCenterNet(TrainConfig(), 'cpu', 'late_fusion', 'regnety_032', 'regnety_032', use_velocity=False)
-    a, b = mine.state_dict(), ref.state_dict()
-    assert list(a.keys()) == list(b.keys()) and all(a[k].shape == b[k].shape for k in a)
-    names = [(n, tuple(p.shape)) for n, p in list(ref.named_parameters()) + list(ref.named_buffers())]
-    ref.load_state_dict(O.deterministic_state(names, seed=6), strict=False)
+    assert_same_state_dict(mine, 'late_fusion')
+    P = O.deterministic_state(ref_names('late_fusion'), seed=6)
     batch = O.synthetic_batch(1, seed=4)
-    P = {k: v.clone() for k, v in ref.state_dict().items()}
     with torch.no_grad():
-        want = ref(batch['rgb'], batch['lidar'], ego_waypoint=batch['ego_waypoint'], target_point=batch['target_point'],
-                   target_point_image=batch['target_point_image'], ego_vel=batch['ego_vel'], bev=batch['bev'], label=batch['label'],
-                   depth=batch['depth'], semantic=batch['semantic'])
         got = O.forward(P, batch, O.Cfg, train=True, backbone_name='late_fusion')
-    for k in want:
-        assert abs(float(want[k]) - float(got[k])) <= 1e-6 * max(abs(float(want[k])), 1e-6), k
+    assert_losses(got, 'late_fusion', 1e-6, 1e-6)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_geometric_fusion_oracle_matches_verbatim_reference():
     """BASELINE config 4 (geometric_fusion.py): oracle restatement vs the reference module, batch 2 so that the
     reference's B x B gather + diagonal (geometric_fusion.py:145-147) is exercised with distinct per-sample indices."""
-    m = ref_import.load()
-    cfg = m['config'].GlobalConfig(setting='eval')
-    cfg.use_target_point_image = True
-    torch.manual_seed(0)
-    ref = m['model'].LidarCenterNet(cfg, 'cpu', 'geometric_fusion', 'regnety_032', 'regnety_032', use_velocity=False).train()
-    names = [(n, tuple(p.shape)) for n, p in list(ref.named_parameters()) + list(ref.named_buffers())]
-    ref.load_state_dict(O.deterministic_state(names, seed=8), strict=False)
+    P = O.deterministic_state(ref_names('geometric_fusion'), seed=8)
     batch = O.synthetic_batch(2, seed=5)
     batch['bev_points'], batch['cam_points'] = O.synthetic_correspondences(2, seed=5)
-    P = {k: v.clone() for k, v in ref.state_dict().items()}
     with torch.no_grad():
-        want = ref(batch['rgb'], batch['lidar'], ego_waypoint=batch['ego_waypoint'], target_point=batch['target_point'],
-                   target_point_image=batch['target_point_image'], ego_vel=batch['ego_vel'], bev=batch['bev'], label=batch['label'],
-                   depth=batch['depth'], semantic=batch['semantic'], bev_points=batch['bev_points'], cam_points=batch['cam_points'])
         got = O.forward(P, batch, O.Cfg, train=True, backbone_name='geometric_fusion')
-    assert set(want) == set(got)
-    for k in want:
-        # fp32: the gather-sum adds the 5 correspondences in a different order than the reference's diagonal/permute/sum
-        assert abs(float(want[k]) - float(got[k])) <= 1e-4 * max(abs(float(want[k])), 1e-3), (k, float(want[k]), float(got[k]))
+    # fp32: the gather-sum adds the 5 correspondences in a different order than the reference's diagonal/permute/sum
+    assert_losses(got, 'geometric_fusion', 1e-4, 1e-3)
 
 
-def _ref_eval_model(m, backbone, seed):
-    cfg = m['config'].GlobalConfig(setting='eval')
-    cfg.use_target_point_image = True
-    cfg.n_layer = 4
-    torch.manual_seed(0)
-    ref = m['model'].LidarCenterNet(cfg, 'cpu', backbone, 'regnety_032', 'regnety_032', use_velocity=False)
-    names = [(n, tuple(p.shape)) for n, p in list(ref.named_parameters()) + list(ref.named_buffers())]
-    ref.load_state_dict(O.deterministic_state(names, seed=seed), strict=False)
-    return ref.eval()
-
-
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_decode_heatmap_oracle_matches_reference_head():
     """model.py:376-497 (get_bboxes / decode_heatmap) on seeded maps with plateaus, saturated peaks and border maxima."""
-    m = ref_import.load()
-    ref = _ref_eval_model(m, 'transFuser', 3)
     g = torch.Generator().manual_seed(21)
     for case in range(3):
         B = 2
@@ -167,10 +138,9 @@ def test_decode_heatmap_oracle_matches_reference_head():
         if case == 2:
             heat = heat * (heat > 0.995)             # fewer than k peaks: the tail of the top-k is zeros
         preds = [heat] + [torch.randn(B, c, 64, 64, generator=g) for c in (2, 2, 12, 1, 1, 2)]
-        want = ref.head.get_bboxes(*[[p] for p in preds])
         got_boxes, got_labels = O.decode_heatmap(preds, 12)
         for b in range(B):
-            wb, wl = want[b]
+            wb, wl = torch.from_numpy(REF['decode_%d_%d_boxes' % (case, b)]), torch.from_numpy(REF['decode_%d_%d_labels' % (case, b)])
             keep = wb[:, -1] > 0                     # rows with score 0 are an arbitrary choice among equal zeros
             if case != 1:                            # (ties between equal positive scores are ordered arbitrarily by topk)
                 assert torch.equal(wb[keep], got_boxes[b][keep]) and torch.equal(wl[keep], got_labels[b][keep])
@@ -178,44 +148,24 @@ def test_decode_heatmap_oracle_matches_reference_head():
                 assert torch.equal(wb[:, -1], got_boxes[b][:, -1])
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_forward_ego_oracle_matches_verbatim_reference():
     """model.py:685-731 in eval mode (running-stat BN, no dropout): waypoints, decoded boxes, ego-frame box corners."""
-    m = ref_import.load()
-    ref = _ref_eval_model(m, 'transFuser', 9)
     batch = O.synthetic_batch(1, seed=6)
-    P = {k: v.clone() for k, v in ref.state_dict().items()}
+    P = O.deterministic_state(ref_names('transFuser'), seed=9)
     with torch.no_grad():
-        wp, boxes = ref.forward_ego(batch['rgb'], batch['lidar'], batch['target_point'], batch['target_point_image'], batch['ego_vel'])
         got_wp, got_boxes, raw = O.forward_ego(P, batch, O.Cfg)
-    assert torch.allclose(wp, got_wp, rtol=1e-5, atol=1e-5)
+    assert torch.allclose(torch.from_numpy(REF['ego_wp']), got_wp, rtol=1e-5, atol=1e-5)
+    boxes = list(zip(REF['ego_boxes'], REF['ego_brake'], REF['ego_conf']))
     assert len(boxes) == len(got_boxes) and len(boxes) > 0, (len(boxes), len(got_boxes), float(raw[0, 0, -1]))
     for (a, abrake, aconf), (b, bbrake, bconf) in zip(boxes, got_boxes):
         assert np.allclose(a, b, rtol=1e-5, atol=1e-5) and abrake == bbrake and abs(aconf - bconf) < 1e-6
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_latent_tf_oracle_matches_verbatim_reference():
     """latentTF.py (positional grid instead of the LiDAR histogram): the 11 training losses, eval mode for the dropouts."""
-    m = ref_import.load()
-    cfg = m['config'].GlobalConfig(setting='eval')
-    cfg.use_target_point_image = True
-    cfg.n_layer = 4
-    torch.manual_seed(0)
-    ref = m['model'].LidarCenterNet(cfg, 'cpu', 'latentTF', 'regnety_032', 'regnety_032', use_velocity=False)
-    names = [(n, tuple(p.shape)) for n, p in list(ref.named_parameters()) + list(ref.named_buffers())]
-    ref.load_state_dict(O.deterministic_state(names, seed=12), strict=False)
-    for mode in (True, False):
-        ref.train(mode)
-        for mod in ref.modules():
-            if isinstance(mod, torch.nn.Dropout):
-                mod.p = 0.0
+    P = O.deterministic_state(ref_names('latentTF'), seed=12)
+    for mode in (True, False):        # the train-mode pass updates P's BatchNorm running statistics, as it does the reference's
         batch = O.synthetic_batch(2, seed=7)
-        P = {k: v.clone() for k, v in ref.state_dict().items()}
         with torch.no_grad():
-            want = ref(batch['rgb'].clone(), batch['lidar'].clone(), ego_waypoint=batch['ego_waypoint'], target_point=batch['target_point'],
-                       target_point_image=batch['target_point_image'], ego_vel=batch['ego_vel'], bev=batch['bev'], label=batch['label'],
-                       depth=batch['depth'], semantic=batch['semantic'])
             got = O.forward(P, batch, O.Cfg, train=mode, backbone_name='latentTF')
-        for k in want:
-            assert abs(float(want[k]) - float(got[k])) <= 1e-5 * max(abs(float(want[k])), 1e-3), (mode, k, float(want[k]), float(got[k]))
+        assert_losses(got, 'latentTF_%d' % mode, 1e-5, 1e-3)

@@ -1,6 +1,6 @@
-"""GPU input pipeline (SURVEY.md §8f rank 2; data.py:103-356). CPU: the numpy oracle against the reference's own functions
-(exec'd from data.py with the real OpenCV) and against the committed fixture; host-side pose algebra of the product against
-the reference. GPU: the three kernels against the oracle — bytes / indices / histogram counts bit-exact."""
+"""GPU input pipeline (SURVEY.md §8f rank 2; data.py:103-356). CPU: the numpy oracle against the outputs of the reference's own
+functions (exec'd from data.py with the real OpenCV; tests/golden/reference_checks.npz) and against the committed fixture;
+host-side pose algebra of the product against the reference. GPU: the three kernels against the oracle — bytes / indices / histogram counts bit-exact."""
 import os
 
 import numpy as np
@@ -8,7 +8,8 @@ import pytest
 import torch
 
 from oracle import pipeline_oracle as PO
-from oracle import bev_oracle, ref_import
+from oracle import bev_oracle
+from oracle.make_golden_reference import GOLD as REF_GOLD, digest, sample_index
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'pipeline_golden.npz')
 DEV = 'cuda'   # the emulated re-runs (tests/test_widen_emulated.py, tools/emulated_module_checks.py) switch this to 'cpu'
@@ -33,27 +34,22 @@ def _oracle_sample(f, crop=(160, 704), scale=1, img_width=320):
                 target_point_image=PO.draw_target_point(f['target_point']).astype(np.float32), T=T, shift=shift)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_pipeline_oracle_matches_reference_functions():
-    fn = ref_import.load_data_fns(['align', 'draw_target_point', 'crop_image_cv2', 'crop_seg', 'get_depth', 'lidar_to_histogram_features'])
+    """Bit-exact against the reference's align / lidar_to_histogram_features / crop_image_cv2 / get_depth / crop_seg /
+    draw_target_point on the same inputs (digests of their outputs, oracle/make_golden_reference.py)."""
+    g = np.load(REF_GOLD)
     for seed in range(6):
         f = PO.synthetic_frame(seed)
         shift = f['degree'] / 60 * 320 / 1                                   # data.py:219, config.img_width 320 (float; the crops apply int())
-        want_pts = fn['align'](f['points'], dict(ego_matrix=f['ego_matrix_0']), dict(ego_matrix=f['ego_matrix_1']), degree=f['degree'])
         T = PO.align_transform(f['ego_matrix_0'], f['ego_matrix_1'], f['degree'])
         got_pts = PO.align_points(f['points'], T)
-        assert want_pts.dtype == got_pts.dtype == np.float64 and np.array_equal(want_pts, got_pts)
-        assert np.array_equal(fn['lidar_to_histogram_features'](want_pts), bev_oracle.lidar_to_histogram_features(got_pts))
-        assert np.array_equal(fn['crop_image_cv2'](f['rgb'], crop=(160, 704), crop_shift=shift), PO.crop_rgb(f['rgb'], (160, 704), shift))
-        d = fn['get_depth'](fn['crop_image_cv2'](f['depth'], crop=(160, 704), crop_shift=shift))
-        assert np.array_equal(d, PO.depth_from_rgb(PO.crop_rgb(f['depth'], (160, 704), shift)))
-        s = np.uint8(CONVERTER)[fn['crop_seg'](f['seg'], crop=(160, 704), crop_shift=shift)]
-        assert np.array_equal(s, PO.seg_classes(f['seg'], CONVERTER, (160, 704), shift))
-    rng = np.random.default_rng(0)
-    pts = [rng.uniform(-40, 40, 2) for _ in range(300)] + [np.array([x, y]) for x in (-16.2, -16.0, 15.9, 16.0, 16.1) for y in (-1.4, -1.3, 30.6, 30.7, 30.8)]
-    pts += [np.array([1e12, -1e12]), np.array([0.0, 0.0])]
-    for tp in pts:
-        assert np.array_equal(fn['draw_target_point'](tp), PO.draw_target_point(tp)), tp
+        assert got_pts.dtype == np.float64 and digest(got_pts) == str(g['pipe_%d_align' % seed]), seed
+        assert digest(bev_oracle.lidar_to_histogram_features(got_pts)) == str(g['pipe_%d_lidar' % seed]), seed
+        assert digest(PO.crop_rgb(f['rgb'], (160, 704), shift)) == str(g['pipe_%d_rgb' % seed]), seed
+        assert digest(PO.depth_from_rgb(PO.crop_rgb(f['depth'], (160, 704), shift))) == str(g['pipe_%d_depth' % seed]), seed
+        assert digest(PO.seg_classes(f['seg'], CONVERTER, (160, 704), shift)) == str(g['pipe_%d_seg' % seed]), seed
+    for tp, want in zip(g['target_points'], g['target_point_images']):
+        assert digest(PO.draw_target_point(tp)) == str(want), tp
 
 
 def test_pipeline_oracle_matches_golden():
@@ -64,17 +60,17 @@ def test_pipeline_oracle_matches_golden():
             assert np.array_equal(o[k], g['%s_%d' % (k, seed)]), (k, seed)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference checkout not present (GPU box)')
 def test_product_pose_algebra_matches_reference():
-    """transfuser_b200.pipeline.align_transform (host numpy, like the reference) applied the reference's way == align()."""
+    """transfuser_b200.pipeline.align_transform (host numpy, like the reference) applied the reference's way == align()
+    (a seeded sample of align()'s points, and the digest of the histogram of all of them)."""
     from transfuser_b200 import pipeline
-    fn = ref_import.load_data_fns(['align'])
+    g = np.load(REF_GOLD)
     for seed in range(4):
         f = PO.synthetic_frame(seed)
         T = pipeline.align_transform(f['ego_matrix_0'], f['ego_matrix_1'], f['degree'])
-        want = fn['align'](f['points'], dict(ego_matrix=f['ego_matrix_0']), dict(ego_matrix=f['ego_matrix_1']), degree=f['degree'])
-        assert np.allclose(PO.align_points(f['points'], T), want, rtol=0, atol=1e-9)
-        assert np.array_equal(bev_oracle.lidar_to_histogram_features(PO.align_points(f['points'], T)), bev_oracle.lidar_to_histogram_features(want))
+        got = PO.align_points(f['points'], T)
+        assert np.allclose(got[sample_index(len(got), seed)], g['pipe_%d_align_sample' % seed], rtol=0, atol=1e-9)
+        assert digest(bev_oracle.lidar_to_histogram_features(got)) == str(g['pipe_%d_lidar' % seed])
     assert pipeline.crop_shift_pixels(-13.7, 320, 1) == int(-13.7 / 60 * 320 / 1)
 
 

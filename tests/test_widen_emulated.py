@@ -1,4 +1,4 @@
-"""The kernel-level GPU tests of tests/test_widen.py and tests/test_pipeline.py (first confirmed on a B200 in round 2), executed at their full sizes on the CPU emulation of the unchanged kernel sources — see
+"""The kernel-level GPU tests of tests/test_widen.py and tests/test_pipeline.py, executed at their full sizes on the CPU emulation of the unchanged kernel sources — see
 tests/cuda_emul/ and tests/test_ops_emulated.py. The module-level ones (whole networks) are too slow for the emulation inside
 the test suite; tools/emulated_module_checks.py runs them by hand. Test infrastructure only."""
 import pytest

@@ -1,5 +1,5 @@
 """One training forward + backward of the whole LidarCenterNet in the bf16 tensor-core MODE on the CPU (build container, no GPU):
-every CUDA-core kernel runs on the emulation (tests/cuda_emul/), the three tcgen05 entry points are torch stand-ins written from
+every CUDA-core kernel runs on the emulation (tests/cuda_emul/), the tensor-core entry points are torch stand-ins written from
 their C-ABI contract (tests/cuda_emul/tc_standins.py). Run twice on the same weights and batch — with the host-side options of
 DESIGN.md 4b (sidecars, fused SE backward, q|k|v pack, BatchNorm+add+ReLU, batched weight pack) on and off — and against the fp32
 CPU oracle. By hand:   python tools/emulated_bf16_step.py [transFuser|late_fusion]      (tens of minutes; test infrastructure)"""

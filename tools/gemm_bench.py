@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM on the shapes of the training step (CUDA events, L2 flushed between launches)."""
+"""Micro-benchmark of the tensor-core GEMM on the shapes of the training step (CUDA events, L2 flushed between launches)."""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -33,5 +33,5 @@ for ta, tb, M, N, K, splits, tag in SHAPES:
         tag, ta, tb, M, N, K, t * 1e3, 2.0 * M * N * K / (t * 1e-3) / 1e12, err, '' if err < 1e-3 else '  <-- WRONG')
     print(line, flush=True)
     out.append(line)
-os.makedirs('gpurun_out', exist_ok=True)
-open('gpurun_out/gemm_bench_%s.txt' % (os.environ.get('TFB_GEMM_BN') or ('model' + os.environ['TFB_GEMM_TILE_MODEL'] if 'TFB_GEMM_TILE_MODEL' in os.environ else 'auto')), 'w').write('\n'.join(out) + '\n')
+os.makedirs('tools_out', exist_ok=True)
+open('tools_out/gemm_bench_%s.txt' % (os.environ.get('TFB_GEMM_BN') or ('model' + os.environ['TFB_GEMM_TILE_MODEL'] if 'TFB_GEMM_TILE_MODEL' in os.environ else 'auto')), 'w').write('\n'.join(out) + '\n')

@@ -34,5 +34,5 @@ for (M, N, K) in [(128, 64, 32), (128, 128, 32), (128, 128, 64), (256, 128, 256)
             line = '%-18s M=%5d N=%5d K=%5d ta=%d tb=%d  relerr=%s nan=%s' % (name, M, N, K, ta, tb, err, nan)
             print(line, flush=True)
             res.append(line)
-os.makedirs('gpurun_out', exist_ok=True)
-open('gpurun_out/gemm_probe.txt', 'w').write('\n'.join(res) + '\n')
+os.makedirs('tools_out', exist_ok=True)
+open('tools_out/gemm_probe.txt', 'w').write('\n'.join(res) + '\n')

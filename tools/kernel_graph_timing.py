@@ -3,7 +3,7 @@
 Runs one eager step, records every call of the chosen C-ABI entry point with its arguments (tensors kept alive), captures exactly
 those launches — in their original order, same operands — into ONE CUDA graph and times the replay with CUDA events. The eager
 per-call timing of bench.py includes the ~15 us Python launch path whenever the GPU is ahead of the host, which inflates the
-average of kernels shorter than that; this number does not. Writes gpurun_out/kernel_graph_timing_<name>.txt."""
+average of kernels shorter than that; this number does not. Writes tools_out/kernel_graph_timing_<name>.txt."""
 import argparse
 import os
 import sys
@@ -80,8 +80,8 @@ def main():
         gb = byts / (ms * 1e-3) / 1e9
         lines.append('algorithmic %.1f MB per step -> %.1f GB/s = %.4f of the HBM peak %.1f' % (byts / 1e6, gb, gb / pk['hbm_gbs'], pk['hbm_gbs']))
     print('\n'.join(lines))
-    os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
-    open(os.path.join(ROOT, 'gpurun_out', 'kernel_graph_timing_%s.txt' % a.name), 'w').write('\n'.join(lines) + '\n')
+    os.makedirs(os.path.join(ROOT, 'tools_out'), exist_ok=True)
+    open(os.path.join(ROOT, 'tools_out', 'kernel_graph_timing_%s.txt' % a.name), 'w').write('\n'.join(lines) + '\n')
 
 
 if __name__ == '__main__':

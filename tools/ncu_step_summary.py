@@ -2,8 +2,8 @@
 (bench.py brackets its instrumented step with cudaProfilerStart / Stop) into a per-kernel table and the DRAM-traffic JSON bench.py reads for `roofline.traffic`.
 
     ncu --profile-from-start off --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum \\
-        --clock-control none --csv --log-file gpurun_out/launches.csv python bench.py --steps 1 --warmup 3 --graph 0 --no-cpu-baseline
-    python tools/ncu_step_summary.py gpurun_out/launches.csv profiles/rN_ncu_launch_summary.txt profiles/rN_ncu_traffic.json
+        --clock-control none --csv --log-file tools_out/launches.csv python bench.py --steps 1 --warmup 3 --graph 0 --no-cpu-baseline
+    python tools/ncu_step_summary.py tools_out/launches.csv tools_out/ncu_launch_summary.txt tools_out/ncu_traffic.json
 """
 import collections
 import csv

@@ -1,6 +1,6 @@
 """Condenses an `ncu --page raw --csv` dump into one line per launch: kernel, grid, duration, DRAM bytes, DRAM / tensor-pipe
-utilisation, achieved occupancy, registers — the per-kernel evidence table committed under profiles/.
-    ncu -i gpurun_out/r2_kernels.ncu-rep --page raw --csv > raw.csv ; python tools/ncu_summarize.py raw.csv > profiles/r2_ncu_kernels.txt"""
+utilisation, achieved occupancy, registers — the per-kernel evidence table.
+    ncu -i tools_out/kernels.ncu-rep --page raw --csv > raw.csv ; python tools/ncu_summarize.py raw.csv > tools_out/ncu_kernels.txt"""
 import csv
 import sys
 

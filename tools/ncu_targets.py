@@ -1,5 +1,5 @@
 """Representative launches of every hot kernel of the training step at its batch-10 shapes, for ONE `ncu --set full` capture:
-    ncu --set full --clock-control none --import-source on -o gpurun_out/r2_kernels python tools/ncu_targets.py
+    ncu --set full --clock-control none --import-source on -o tools_out/kernels python tools/ncu_targets.py
 Each section runs forward + backward of a product op (C-ABI kernels through transfuser_b200.ops), so the capture holds the real
 kernels with the real operand shapes: GPT GEMMs (C = 1512), trunk 1x1 GEMMs with BatchNorm statistics in the epilogue, grouped 3x3
 convs (stride 1 and 2), fused attention, BatchNorm forward / backward, squeeze-excite, AdamW, BEV histogram, bilinear upsample."""

@@ -1,4 +1,4 @@
-"""ctypes binding of the C-ABI in include/tfb200.h (libtfb200.so, hand-written sm_100a CUDA).
+"""ctypes binding of the C-ABI in include/tfb200.h (libtfb200.so, hand-written sm_90a CUDA).
 
 There is deliberately NO fallback: if the library is missing or a kernel returns an error the call raises.
 Signatures are parsed from the header so the header stays the single source of truth for the boundary."""

@@ -1,10 +1,10 @@
-"""B200-native `TransfuserBackbone` — drop-in for /root/reference/team_code_transfuser/transfuser.py:7-211.
+"""H100-native `TransfuserBackbone` — drop-in for team_code_transfuser/transfuser.py:7-211.
 
 Same constructor signature, same `forward(image, lidar, velocity) -> ((p2, p3, p4, p5), image_features_grid,
 fused_features)` contract (NCHW fp32 in / out), and the same parameter / buffer names and shapes as the reference
 (including the alias keys created by ImageCNN / LidarEncoder, transfuser.py:383-393, 475-486), so reference checkpoints
 load unchanged. The nn.Conv2d / nn.BatchNorm2d / nn.Linear / nn.LayerNorm objects below are *parameter containers only*:
-their forward is never called — every op runs through transfuser_b200.ops (hand-written sm_100a kernels, NHWC inside).
+their forward is never called — every op runs through transfuser_b200.ops (hand-written sm_90a kernels, NHWC inside).
 
 The RegNetY-3.2GF definition (timm 0.5.4 `regnety_032`: stem 32, widths 72/216/576/1512, depths 2/5/13/1, group width 24,
 SE ratio 0.25) is restated from timm's published config; timm itself is not a dependency."""
@@ -342,7 +342,7 @@ class _PlainEncoder(nn.Module):
 
 
 class LateFusionBackbone(nn.Module):
-    """B200-native drop-in for /root/reference/team_code_transfuser/late_fusion.py:5-111 (BASELINE config 5): two independent
+    """H100-native drop-in for team_code_transfuser/late_fusion.py:5-111 (BASELINE config 5): two independent
     RegNetY trunks, 1x1 channel reduction, global pools summed, FPN top-down on the LiDAR grid. Same parameter names."""
 
     def __init__(self, config, image_architecture='resnet34', lidar_architecture='resnet18', use_velocity=0):
@@ -424,7 +424,7 @@ def _mlp3(hid):
 
 
 class GeometricFusionBackbone(nn.Module):
-    """B200-native drop-in for /root/reference/team_code_transfuser/geometric_fusion.py:7-296 (BASELINE config 4): at each of
+    """H100-native drop-in for team_code_transfuser/geometric_fusion.py:7-296 (BASELINE config 4): at each of
     the 4 trunk scales, features of one modality are pooled to its anchor grid, gathered at 5 projected correspondences per
     cell of the other modality's grid, summed, passed through a 3-layer MLP and added back at full resolution.
 
@@ -523,7 +523,7 @@ class GeometricFusionBackbone(nn.Module):
 
 
 class latentTFBackbone(TransfuserBackbone):
-    """B200-native drop-in for /root/reference/team_code_transfuser/latentTF.py:8-217: the TransFuser architecture with the two
+    """H100-native drop-in for team_code_transfuser/latentTF.py:8-217: the TransFuser architecture with the two
     LiDAR histogram channels replaced by a fixed positional grid in [-1, 1] (latentTF.py:132-137; the target-point channel is
     kept). Same kernels and schedule as TransfuserBackbone; the only differences are the input assembly and the parameter
     names of the LiDAR stem (its encoder deletes the whole `stem`, latentTF.py:195-196)."""

@@ -1,7 +1,7 @@
-"""GPU drop-in for `lidar_to_histogram_features` (/root/reference/team_code_transfuser/data.py:446-470).
+"""GPU drop-in for `lidar_to_histogram_features` (team_code_transfuser/data.py:446-470).
 
 Same name, same argument meaning (an (N, >=4) point array: x, y, z, intensity) and same result
-((2, 256, 256) float32, channel 0 = above, channel 1 = below), computed by the sm_100a kernel in csrc/bev_hist.cu."""
+((2, 256, 256) float32, channel 0 = above, channel 1 = below), computed by the sm_90a kernel in csrc/bev_hist.cu."""
 import numpy as np
 import torch
 

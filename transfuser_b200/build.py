@@ -1,6 +1,6 @@
-"""In-tree build of the sm_100a CUDA library (libtfb200.so) with nvcc — no torch headers, no JIT cache.
+"""In-tree build of the sm_90a CUDA library (libtfb200.so) with nvcc — no torch headers, no JIT cache.
 
-The built .so is git-ignored but travels to the GPU box with the gpurun snapshot."""
+The objects (csrc/build/) and the .so are build products: git-ignored, rebuilt whenever a source, a header or the flags change."""
 import hashlib
 import os
 import subprocess
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, 'build')
 LIB = os.path.join(HERE, 'libtfb200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fvisibility=hidden',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fvisibility=hidden',
          '--expt-relaxed-constexpr', '-I', CSRC, '-I', os.path.join(os.path.dirname(HERE), 'include')]
 
 

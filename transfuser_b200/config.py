@@ -1,7 +1,7 @@
-"""The GlobalConfig fields (/root/reference/team_code_transfuser/config.py:3-204) that the training hot path reads, with
+"""The GlobalConfig fields (team_code_transfuser/config.py:3-204) that the training hot path reads, with
 train.py's CLI defaults applied (train.py:50-61: regnety_032 trunks, n_layer 4, use_velocity 0, use_target_point_image 1).
 The reference's own `GlobalConfig` instance works unchanged with transfuser_b200.LidarCenterNet; this class exists so that
-bench.py / smoke() / the GPU tests can run where /root/reference is absent."""
+bench.py / smoke() / the GPU tests can run where no reference checkout exists."""
 
 
 class TrainConfig:

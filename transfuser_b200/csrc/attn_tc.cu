@@ -1,16 +1,18 @@
-// Fused multi-head self-attention on the tcgen05 tensor cores (forward and backward) for the GPT fusion blocks
+// Fused multi-head self-attention on the wgmma tensor cores (forward and backward) for the GPT fusion blocks
 // (reference: SelfAttention.forward, transfuser.py:510-527: q k^T / sqrt(hs) -> softmax -> attn_drop -> @ v; T = 174 tokens,
-// 4 heads, head sizes 18 / 54 / 144 / 378). Nothing of size T x T ever reaches HBM: scores live in TMEM, probabilities go
-// through shared memory as the bf16 A operand of the second product, the softmax is one thread per row on the TMEM lanes.
+// 4 heads, head sizes 18 / 54 / 144 / 378). Nothing of size T x T ever reaches HBM: scores live in the wgmma register
+// accumulators, probabilities go through shared memory as the bf16 A operand of the second product.
 //
-// One CTA = one 128-row tile of one (batch, head). Three modes share the kernel body:
-//   FWD   rows = queries : S = Q K^T (TMEM) -> P = softmax(scale S), Pd = dropout(P) (bf16, smem) -> O = Pd V ; saves the
-//                          row log-sum-exp for the backward pass
-//   BWD_Q rows = queries : S = Q K^T, dPd = dO V^T (both TMEM) -> dS = scale P (dPd drop - D) (smem) -> dQ = dS K
-//   BWD_K rows = keys    : S^T = K Q^T, dPd^T = V dO^T (TMEM) -> Pd^T (smem) -> dV = Pd^T dO ; dS^T (smem) -> dK = dS^T Q
-// (P is recomputed from the saved log-sum-exp; D_i = sum_d dO_id O_id comes from a small pre-pass.)
+// One CTA = one 128-row tile of one (batch, head); warpgroup g (threads 128g..128g+127) owns rows [64g, 64g + 64).
+// Three modes share the kernel body:
+//   FWD   rows = queries : S = Q K^T (registers, all 192 columns) -> P = softmax(scale S), Pd = dropout(P) (bf16, smem) -> O = Pd V ;
+//                          saves the row log-sum-exp for the backward pass
+//   BWD_Q rows = queries : S = Q K^T, dPd = dO V^T -> dS = scale P (dPd drop - D) (smem) -> dQ = dS K
+//   BWD_K rows = keys    : S^T = K Q^T, dPd^T = V dO^T -> Pd^T and dS^T (smem) -> dV = Pd^T dO ; dK = dS^T Q
+// (P is recomputed from the saved log-sum-exp; D_i = sum_d dO_id O_id comes from a small pre-pass.) The backward score products
+// run in two 96-column halves so that both accumulators fit the register file.
 // Operands are staged by all threads into 128B-swizzled shared memory (the head slices of the packed [B*T, 3C] q|k|v buffer
-// start at 4-byte-aligned columns, which rules out TMA boxes) and described to tcgen05.mma with the same K-major / MN-major
+// start at 4-byte-aligned columns, which rules out TMA boxes) and described to wgmma with the same K-major / MN-major
 // shared-memory descriptors as gemm_tc.cu. fp32 or bf16 inputs (converted while staging), fp32 accumulation.
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -18,16 +20,20 @@
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kRowsX = 128;                 // tile rows (UMMA M)
+constexpr int kRowsX = 128;                 // tile rows (two wgmma M = 64 halves)
 constexpr int kRowsY = 192;                 // padded rows of the column operand (T <= 192)
+constexpr int kHalf = 96;                   // score columns per backward pass
 constexpr int kXBytes = kRowsX * 128;       // one 64-column bf16 chunk of the row operand
 constexpr int kYBytes = kRowsY * 128;       // one 64-column bf16 chunk of the column operand
-constexpr int kStageBytes = 2 * (kXBytes + kYBytes);   // X1 | Y1 | X2 | Y2 (the second pair is unused in FWD)
+constexpr int kYHalfBytes = kHalf * 128;
+// one streaming stage: X1 | Y1 (FWD: 192 rows, BWD: 96 rows) | X2 | Y2 (BWD only)
+constexpr int kOffY1 = kXBytes, kOffX2 = kXBytes + kYHalfBytes, kOffY2 = 2 * kXBytes + kYHalfBytes;
+constexpr int kStageBytes = 2 * (kXBytes + kYHalfBytes);         // 57344 (>= kXBytes + kYBytes of the forward stage)
 constexpr int kMatBytes = 3 * kXBytes;      // the 128 x 192 bf16 probability / score-gradient matrix (3 K chunks of 64)
 constexpr int kZBuf = 2 * kYBytes;          // two 64-wide chunks of the MN-major B operand of the second product
-constexpr int kSmemStages = 2 * kStageBytes;                     // 163840: two streaming stages; later three Z buffers
-constexpr int kSmemTotal = kSmemStages + kMatBytes + 2048 + 1024;  // + barriers / row statistics + alignment slack
-constexpr uint32_t kAcc1 = 0, kAcc2 = 192, kOut = 384;           // TMEM columns
+constexpr int kSmemStages = 2 * kStageBytes;                     // two streaming stages; later two Z buffers
+constexpr int kSmemTotal = kSmemStages + 2 * kMatBytes + 2 * kRowsY * 4 + 1024;  // + Pd^T / dS^T (BWD_K) + column statistics + slack
+static_assert(kXBytes + kYBytes <= kStageBytes && 2 * kZBuf <= kSmemStages, "attention shared-memory layout");
 
 enum { MODE_FWD = 0, MODE_BWD_Q = 1, MODE_BWD_K = 2 };
 
@@ -45,8 +51,6 @@ struct Params {
   float scale, p_drop;
   int mode;             // MODE_FWD, or 1 = backward (BWD_K CTAs first, then BWD_Q)
 };
-
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // cheap counter-based keep/drop decision for the attention dropout (forward and backward of THIS kernel regenerate it)
 __device__ __forceinline__ float drop_scale(uint32_t seed_lo, uint32_t seed_hi, uint32_t idx, float p, float keep_scale) {
@@ -151,16 +155,98 @@ __device__ __forceinline__ uint32_t mat_off(int r, int j) {
   return (uint32_t)(c * kXBytes + (r >> 3) * 1024 + (r & 7) * 128 + ((u ^ (r & 7)) << 4) + e * 2);
 }
 
+struct Operand {          // a head slice: columns [col, col + hs) of a row-major matrix
+  const void* src;
+  int bf16;
+  int64_t ld;
+  int col;
+};
+
+// acc1 (+)= X1 Y1^T and, when TWO, acc2 (+)= X2 Y2^T over the head dimension, streamed in 64-wide chunks through two stages:
+// X rows [xrow0, xrow0 + 128) (valid: xrows), Y rows [yrow0, yrow0 + NP) (valid: yrows), both K-major.
+template <int NP, bool TWO>
+__device__ __forceinline__ void score_products(uint8_t* smem, const Operand& x1, const Operand& y1, const Operand& x2, const Operand& y2,
+                                               int64_t xrow0, int xrows, int64_t yrow0, int yrows, int hs, int tid, int wg,
+                                               float (&acc1)[NP / 2], float (&acc2)[NP / 2]) {
+  const int nchunks = (hs + 63) / 64;
+  auto issue_loads = [&](int c) {
+    uint8_t* st = smem + (c & 1) * kStageBytes;
+    const int cv = min(64, hs - c * 64);
+    stage_any(st, x1.src, x1.bf16, x1.ld, xrow0, xrows, kRowsX, x1.col + c * 64, cv, tid, kThreads);
+    stage_any(st + kOffY1, y1.src, y1.bf16, y1.ld, yrow0, yrows, NP, y1.col + c * 64, cv, tid, kThreads);
+    if (TWO) {
+      stage_any(st + kOffX2, x2.src, x2.bf16, x2.ld, xrow0, xrows, kRowsX, x2.col + c * 64, cv, tid, kThreads);
+      stage_any(st + kOffY2, y2.src, y2.bf16, y2.ld, yrow0, yrows, NP, y2.col + c * 64, cv, tid, kThreads);
+    }
+    cp_async_commit();
+  };
+  __syncthreads();                                      // the stages may still be read by the other warpgroup's last MMAs
+  issue_loads(0);
+  for (int c = 0; c < nchunks; ++c) {
+    cp_async_wait_all();
+    tc::fence_async_smem();
+    __syncthreads();                                    // chunk c staged; both warpgroups' MMAs of chunk c - 1 have retired
+    const uint32_t st = tc::smem_u32(smem + (c & 1) * kStageBytes);
+    const int ksteps = (min(64, hs - c * 64) + 15) / 16;
+    tc::fence_acc(acc1);
+    if (TWO) tc::fence_acc(acc2);
+    tc::wgmma_fence();
+    for (int k = 0; k < ksteps; ++k) {
+      const uint32_t accum = (c > 0 || k > 0) ? 1u : 0u;
+      tc::wgmma_bf16<0, 0>(acc1, tc::make_smem_desc(st + wg * 8192 + k * 32, 16, 1024), tc::make_smem_desc(st + kOffY1 + k * 32, 16, 1024), accum);
+      if (TWO)
+        tc::wgmma_bf16<0, 0>(acc2, tc::make_smem_desc(st + kOffX2 + wg * 8192 + k * 32, 16, 1024),
+                             tc::make_smem_desc(st + kOffY2 + k * 32, 16, 1024), accum);
+    }
+    tc::wgmma_commit();
+    if (c + 1 < nchunks) issue_loads(c + 1);            // into the stage of chunk c - 1 (retired): overlaps the MMAs of chunk c
+    tc::wgmma_wait<0>();
+    tc::fence_acc(acc1);
+    if (TWO) tc::fence_acc(acc2);
+  }
+}
+
+// out[64 rows of this warpgroup x NM] = M Z over K = ncols tokens: M (bf16, K-major, 3 chunks of 64 tokens) from the
+// element-wise stage, Z (MN-major: token rows x head-dimension columns, two 64-wide chunks). Columns d < dvalid of the rows
+// with row_ok are scaled by mul[] and written to o32 / o16 (row stride old).
+template <int NM>
+__device__ __forceinline__ void value_product(const uint8_t* mat, const uint8_t* zb, int ncols, int wg, int t128, const bool (&row_ok)[2],
+                                              const int64_t (&orow)[2], const float (&mul)[2], int dvalid, float* o32, __nv_bfloat16* o16) {
+  float o[NM / 2];
+  tc::fence_acc(o);
+  tc::wgmma_fence();
+  const uint32_t sm = tc::smem_u32(mat) + wg * 8192, sz = tc::smem_u32(zb);
+  for (int k = 0; k < ncols / 16; ++k)
+    tc::wgmma_bf16<0, 1>(o, tc::make_smem_desc(sm + (k >> 2) * kXBytes + (k & 3) * 32, 16, 1024), tc::make_smem_desc(sz + k * 2048, kYBytes, 1024),
+                         k > 0 ? 1u : 0u);
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::fence_acc(o);
+#pragma unroll
+  for (int i = 0; i < NM / 2; i += 2) {
+    const int h = (i >> 1) & 1, d = tc::frag_col(t128, i);
+    if (row_ok[h] && d < dvalid) {                      // (dvalid is even)
+      const float a = o[i] * mul[h], b = o[i + 1] * mul[h];
+      if (o32) *reinterpret_cast<float2*>(o32 + orow[h] + d) = make_float2(a, b);
+      if (o16) *reinterpret_cast<__nv_bfloat162*>(o16 + orow[h] + d) = __floats2bfloat162_rn(a, b);
+    }
+  }
+}
+
+__device__ __forceinline__ void store_pair(uint8_t* mat, int r, int j, float a, float b) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+  *reinterpret_cast<__nv_bfloat162*>(mat + mat_off(r, j)) = v;
+}
+
 __global__ void __launch_bounds__(kThreads, 1) attn_tc_kernel(const Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* mat = smem + kSmemStages;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kSmemStages + kMatBytes);   // [0,1]: stage s consumed; [2]: second product done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-  float* stat_a = reinterpret_cast<float*>(smem + kSmemStages + kMatBytes + 64);  // [192] lse of the column tokens (BWD_K)
-  float* stat_b = stat_a + kRowsY;                                                 // [192] D   of the column tokens (BWD_K)
+  uint8_t* mat0 = smem + kSmemStages;                    // Pd (FWD) / dS (BWD_Q) / Pd^T (BWD_K)
+  uint8_t* mat1 = mat0 + kMatBytes;                      // dS^T (BWD_K)
+  float* stat_a = reinterpret_cast<float*>(mat1 + kMatBytes);   // [192] lse of the column tokens (BWD_K)
+  float* stat_b = stat_a + kRowsY;                               // [192] D   of the column tokens (BWD_K)
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, t128 = tid & 127;
   const int T = p.T, nh = p.nh, hs = p.hs, C = p.C;
   const int tiles = (T + kRowsX - 1) / kRowsX;
   int blk = blockIdx.x, mode = MODE_FWD;
@@ -172,257 +258,146 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tc_kernel(const Params p) {
   const int tile = blk % tiles, bh = blk / tiles, h = bh % nh, b = bh / nh;
   const int m0 = tile * kRowsX;
   const int rows_valid = min(kRowsX, T - m0);
-  const int ncols = (T + 15) & ~15;                     // UMMA N of the score products (and K extent of the second product)
+  const int ncols = (T + 15) & ~15;                     // K extent of the second product
   const int64_t tok0 = (int64_t)b * T;                  // first token row of this batch element
   const int64_t ld3 = 3 * (int64_t)C;
-  const bool bwd = mode != MODE_FWD;
-
-  if (tid == 0) {
-    for (int i = 0; i < 3; ++i) tc::mbar_init(&bars[i], 1);
-    tc::mbar_fence_init();
-  }
-  if (warp == 0) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  uint32_t ph_stage[2] = {0u, 0u}, ph_out = 0u;
 
   // column offsets (elements) of the operands inside their matrices
   const int colq = h * hs, colk = C + h * hs, colv = 2 * C + h * hs, coly = h * hs;
-  // first product(s): acc1 = X1 Y1^T (rows x ncols), acc2 = X2 Y2^T, streamed over 64-wide chunks of the head dimension
-  //   FWD / BWD_Q: X1 = Q tile, Y1 = K;  BWD_Q also X2 = dO tile, Y2 = V.   BWD_K: X1 = K tile, Y1 = Q, X2 = V tile, Y2 = dO.
-  const int x1col = mode == MODE_BWD_K ? colk : colq, y1col = mode == MODE_BWD_K ? colq : colk;
-  const int nchunks = (hs + 63) / 64;
-  auto issue_loads = [&](int c) {
-    uint8_t* st = smem + (c & 1) * kStageBytes;
-    const int cv = min(64, hs - c * 64);
-    stage_any(st, p.qkv, p.in_bf16, ld3, tok0 + m0, rows_valid, kRowsX, x1col + c * 64, cv, tid, kThreads);
-    stage_any(st + kXBytes, p.qkv, p.in_bf16, ld3, tok0, T, kRowsY, y1col + c * 64, cv, tid, kThreads);
-    if (mode == MODE_BWD_Q) {
-      stage_any(st + kXBytes + kYBytes, p.dy, p.dy_bf16, C, tok0 + m0, rows_valid, kRowsX, coly + c * 64, cv, tid, kThreads);
-      stage_any(st + 2 * kXBytes + kYBytes, p.qkv, p.in_bf16, ld3, tok0, T, kRowsY, colv + c * 64, cv, tid, kThreads);
-    } else if (mode == MODE_BWD_K) {
-      stage_any(st + kXBytes + kYBytes, p.qkv, p.in_bf16, ld3, tok0 + m0, rows_valid, kRowsX, colv + c * 64, cv, tid, kThreads);
-      stage_any(st + 2 * kXBytes + kYBytes, p.dy, p.dy_bf16, C, tok0, T, kRowsY, coly + c * 64, cv, tid, kThreads);
-    }
-    cp_async_commit();
-  };
-  issue_loads(0);
-  for (int c = 0; c < nchunks; ++c) {
-    const int s = c & 1;
-    if (c + 1 < nchunks) {
-      // the copies of chunk c + 1 go out before chunk c is consumed: its stage was last read by the MMAs of chunk c - 1
-      if (c >= 1) { tc::mbar_wait(&bars[s ^ 1], ph_stage[s ^ 1]); ph_stage[s ^ 1] ^= 1u; }
-      issue_loads(c + 1);
-      cp_async_wait_group<1>();                        // everything but the newest group (chunk c + 1) has landed
-    } else {
-      cp_async_wait_all();
-    }
-    uint8_t* st = smem + s * kStageBytes;
-    const int cv = min(64, hs - c * 64);
-    fence_async_smem();
-    __syncthreads();
-    if (tid == 0) {
-      tc::fence_after_sync();
-      const uint32_t idesc = tc::make_idesc(1u, 0u, 0u, kRowsX, (uint32_t)ncols);
-      const uint32_t sx1 = tc::smem_u32(st), sy1 = sx1 + kXBytes, sx2 = sy1 + kYBytes, sy2 = sx2 + kXBytes;
-      const int ksteps = (cv + 15) / 16;
-      for (int k = 0; k < ksteps; ++k) {
-        const uint32_t acc = (c > 0 || k > 0) ? 1u : 0u;
-        tc::umma_f16(tmem + kAcc1, tc::make_smem_desc(sx1 + k * 32, 16, 1024), tc::make_smem_desc(sy1 + k * 32, 16, 1024), idesc, acc);
-        if (bwd)
-          tc::umma_f16(tmem + kAcc2, tc::make_smem_desc(sx2 + k * 32, 16, 1024), tc::make_smem_desc(sy2 + k * 32, 16, 1024), idesc, acc);
-      }
-      tc::umma_commit(&bars[s]);
-    }
-  }
-  // drain: every outstanding stage commit (at most two) is waited for exactly once, oldest first
-  // (iteration c waited for chunk c - 1 whenever it prefetched chunk c + 1: chunks 0 .. nchunks - 3 are done with)
-  if (nchunks >= 2) { const int s = nchunks & 1; tc::mbar_wait(&bars[s], ph_stage[s]); ph_stage[s] ^= 1u; }
-  { const int s = (nchunks - 1) & 1; tc::mbar_wait(&bars[s], ph_stage[s]); ph_stage[s] ^= 1u; }
-  tc::fence_after_sync();
+  const Operand Q{p.qkv, p.in_bf16, ld3, colq}, K{p.qkv, p.in_bf16, ld3, colk}, V{p.qkv, p.in_bf16, ld3, colv}, dO{p.dy, p.dy_bf16, C, coly};
 
   const uint32_t seed_lo = (uint32_t)((p.seed_dev ? *p.seed_dev : 0ull) + p.seed_off);
   const uint32_t seed_hi = (uint32_t)(((p.seed_dev ? *p.seed_dev : 0ull) + p.seed_off) >> 32);
   const float keep = p.p_drop > 0.f ? 1.f / (1.f - p.p_drop) : 1.f;
   const float sl2 = p.scale * 1.4426950408889634f;
-  const int r = tid & 127;                               // this thread's tile row = its TMEM lane (warps 0-3; warps 4-7 mirror)
-  const uint32_t lane_addr = ((uint32_t)((warp & 3) * 32)) << 16;
-  const bool row_ok = r < rows_valid;
-  const int tok = m0 + r;                                // token index of this row inside the batch element
-  float inv_sum = 1.f;
+  // the two tile rows of this thread's accumulator fragments (frag_row(t, i) for even / odd i >> 1)
+  int row[2];
+  bool row_ok[2];
+  int tok[2];                                            // token index of the row inside the batch element
+  for (int e = 0; e < 2; ++e) {
+    row[e] = wg * 64 + tc::frag_row(t128, 2 * e);
+    row_ok[e] = row[e] < rows_valid;
+    tok[e] = m0 + row[e];
+  }
+  float mul[2] = {1.f, 1.f};
 
   if (mode == MODE_BWD_K) {                              // per-column statistics of all query tokens
     for (int i = tid; i < kRowsY; i += kThreads) {
       stat_a[i] = i < T ? p.lse[(int64_t)bh * T + i] * 1.4426950408889634f : 0.f;
       stat_b[i] = i < T ? p.dsum[(int64_t)bh * T + i] : 0.f;
     }
-    __syncthreads();
   }
 
-  // second product(s): out[rows x hs] = M Z, M (bf16, smem, K-major, K = ncols tokens) from the element-wise stage, Z MN-major.
+  if (mode == MODE_FWD) {
+    float s[kRowsY / 2];
+    score_products<kRowsY, false>(smem, Q, K, Q, K, tok0 + m0, rows_valid, tok0, T, hs, tid, wg, s, s);
+    float mx[2] = {-INFINITY, -INFINITY}, sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < kRowsY / 2; ++i)
+      if (tc::frag_col(t128, i) < T) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    for (int e = 0; e < 2; ++e) {                        // the 4 lanes of a quad share a row
+      mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 1));
+      mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 2));
+    }
+#pragma unroll
+    for (int i = 0; i < kRowsY / 2; i += 2) {
+      const int e = (i >> 1) & 1, j = tc::frag_col(t128, i);
+      const uint32_t ibase = (uint32_t)(((int64_t)bh * T + tok[e]) * T);
+      float v[2] = {0.f, 0.f};
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        if (j + q < T) {
+          v[q] = exp2f((s[i + q] - mx[e]) * sl2);
+          sum[e] += v[q];
+          if (p.p_drop > 0.f) v[q] *= drop_scale(seed_lo, seed_hi, ibase + j + q, p.p_drop, keep);
+        }
+      }
+      store_pair(mat0, row[e], j, v[0], v[1]);
+    }
+    for (int e = 0; e < 2; ++e) {
+      sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 1);
+      sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 2);
+      mul[e] = 1.f / sum[e];
+      if (row_ok[e] && (t128 & 3) == 0 && p.lse) p.lse[(int64_t)bh * T + tok[e]] = mx[e] * p.scale + logf(sum[e]);
+    }
+  } else {
+    float lse2[2], dsum[2];
+    for (int e = 0; e < 2; ++e) {
+      lse2[e] = (mode == MODE_BWD_Q && row_ok[e]) ? p.lse[(int64_t)bh * T + tok[e]] * 1.4426950408889634f : 0.f;
+      dsum[e] = (mode == MODE_BWD_Q && row_ok[e]) ? p.dsum[(int64_t)bh * T + tok[e]] : 0.f;
+    }
+    for (int hc = 0; hc * kHalf < T; ++hc) {
+      const int cbase = hc * kHalf;
+      float s[kHalf / 2], g[kHalf / 2];
+      if (mode == MODE_BWD_Q)
+        score_products<kHalf, true>(smem, Q, K, dO, V, tok0 + m0, rows_valid, tok0 + cbase, T - cbase, hs, tid, wg, s, g);
+      else
+        score_products<kHalf, true>(smem, K, Q, V, dO, tok0 + m0, rows_valid, tok0 + cbase, T - cbase, hs, tid, wg, s, g);
+#pragma unroll
+      for (int i = 0; i < kHalf / 2; i += 2) {
+        const int e = (i >> 1) & 1, j = cbase + tc::frag_col(t128, i);
+        float o0[2] = {0.f, 0.f}, o1[2] = {0.f, 0.f};
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int c = j + q;
+          if (c >= T) continue;
+          if (mode == MODE_BWD_Q) {                       // rows = queries, columns = keys c
+            const float pr = exp2f(s[i + q] * sl2 - lse2[e]);
+            const float gd = p.p_drop > 0.f ? g[i + q] * drop_scale(seed_lo, seed_hi, (uint32_t)(((int64_t)bh * T + tok[e]) * T) + c, p.p_drop, keep) : g[i + q];
+            o0[q] = p.scale * pr * (gd - dsum[e]);
+          } else {                                        // rows = keys (tok), columns = queries c: S^T and dPd^T
+            const float pr = exp2f(s[i + q] * sl2 - stat_a[c]);
+            const float ds = p.p_drop > 0.f ? drop_scale(seed_lo, seed_hi, (uint32_t)(((int64_t)bh * T + c) * T + tok[e]), p.p_drop, keep) : 1.f;
+            o0[q] = pr * ds;
+            o1[q] = p.scale * pr * (g[i + q] * ds - stat_b[c]);
+          }
+        }
+        store_pair(mat0, row[e], j, o0[0], o0[1]);
+        if (mode == MODE_BWD_K) store_pair(mat1, row[e], j, o1[0], o1[1]);
+      }
+    }
+  }
+
+  // second product(s): out[rows x hs] = M Z, M from the element-wise stage, Z MN-major, in passes of 128 head-dimension columns.
   //   FWD: M = Pd, Z = V -> y.   BWD_Q: M = dS, Z = K -> dQ.   BWD_K: round 0 M = Pd^T, Z = dO -> dV; round 1 M = dS^T, Z = Q -> dK.
   const int nrounds = mode == MODE_BWD_K ? 2 : 1;
   const int npass = (hs + 127) / 128;
   for (int round = 0; round < nrounds; ++round) {
-    const void* zsrc; int z_bf16, zcol; int64_t zld;
+    Operand z;
     int ocol;                                            // output column (in out*_a, leading dimension old)
     int64_t old;
-    if (mode == MODE_FWD)        { zsrc = p.qkv; z_bf16 = p.in_bf16; zld = ld3; zcol = colv; ocol = coly; old = C; }
-    else if (mode == MODE_BWD_Q) { zsrc = p.qkv; z_bf16 = p.in_bf16; zld = ld3; zcol = colk; ocol = colq; old = ld3; }
-    else if (round == 0)         { zsrc = p.dy;  z_bf16 = p.dy_bf16; zld = C;   zcol = coly; ocol = colv; old = ld3; }
-    else                         { zsrc = p.qkv; z_bf16 = p.in_bf16; zld = ld3; zcol = colq; ocol = colk; old = ld3; }
+    if (mode == MODE_FWD)        { z = V;  ocol = coly; old = C; }
+    else if (mode == MODE_BWD_Q) { z = K;  ocol = colq; old = ld3; }
+    else if (round == 0)         { z = dO; ocol = colv; old = ld3; }
+    else                         { z = Q;  ocol = colk; old = ld3; }
+    const uint8_t* mat = round == 0 ? mat0 : mat1;
+    const int64_t orow[2] = {(tok0 + tok[0]) * old + ocol, (tok0 + tok[1]) * old + ocol};
 
-    // ---- element-wise stage (warps 0-3: one thread per row, straight out of TMEM) while warps 4-7 stage the first Z buffer ----
-    if (warp < 4) {
-      if (mode == MODE_FWD) {
-        float mx = -INFINITY;
-        for (int j0 = 0; j0 < ncols; j0 += 16) {
-          float v[16];
-          tc::tmem_ld16(tmem + lane_addr + kAcc1 + j0, v);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) if (j0 + j < T) mx = fmaxf(mx, v[j]);
-        }
-        float sum = 0.f;
-        const uint32_t ibase = (uint32_t)(((int64_t)bh * T + tok) * T);
-        for (int j0 = 0; j0 < ncols; j0 += 16) {
-          float v[16];
-          tc::tmem_ld16(tmem + lane_addr + kAcc1 + j0, v);
-          uint32_t w[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            float e0 = 0.f, e1 = 0.f;
-            if (j0 + j < T)     { e0 = exp2f((v[j] - mx) * sl2);     sum += e0; if (p.p_drop > 0.f) e0 *= drop_scale(seed_lo, seed_hi, ibase + j0 + j, p.p_drop, keep); }
-            if (j0 + j + 1 < T) { e1 = exp2f((v[j + 1] - mx) * sl2); sum += e1; if (p.p_drop > 0.f) e1 *= drop_scale(seed_lo, seed_hi, ibase + j0 + j + 1, p.p_drop, keep); }
-            __nv_bfloat162 bb = __floats2bfloat162_rn(e0, e1);
-            w[j >> 1] = *reinterpret_cast<uint32_t*>(&bb);
-          }
-          *reinterpret_cast<uint4*>(mat + mat_off(r, j0)) = make_uint4(w[0], w[1], w[2], w[3]);
-          *reinterpret_cast<uint4*>(mat + mat_off(r, j0 + 8)) = make_uint4(w[4], w[5], w[6], w[7]);
-        }
-        inv_sum = 1.f / sum;
-        if (row_ok && p.lse) p.lse[(int64_t)bh * T + tok] = mx * p.scale + logf(sum);
-      } else if (mode == MODE_BWD_Q) {
-        const float lse2 = row_ok ? p.lse[(int64_t)bh * T + tok] * 1.4426950408889634f : 0.f;
-        const float dsum = row_ok ? p.dsum[(int64_t)bh * T + tok] : 0.f;
-        const uint32_t ibase = (uint32_t)(((int64_t)bh * T + tok) * T);
-        for (int j0 = 0; j0 < ncols; j0 += 16) {
-          float sv[16], gv[16];
-          tc::tmem_ld16(tmem + lane_addr + kAcc1 + j0, sv);
-          tc::tmem_ld16(tmem + lane_addr + kAcc2 + j0, gv);
-          uint32_t w[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            float d0 = 0.f, d1 = 0.f;
-            if (j0 + j < T) {
-              const float pr = exp2f(sv[j] * sl2 - lse2);
-              const float g = p.p_drop > 0.f ? gv[j] * drop_scale(seed_lo, seed_hi, ibase + j0 + j, p.p_drop, keep) : gv[j];
-              d0 = p.scale * pr * (g - dsum);
-            }
-            if (j0 + j + 1 < T) {
-              const float pr = exp2f(sv[j + 1] * sl2 - lse2);
-              const float g = p.p_drop > 0.f ? gv[j + 1] * drop_scale(seed_lo, seed_hi, ibase + j0 + j + 1, p.p_drop, keep) : gv[j + 1];
-              d1 = p.scale * pr * (g - dsum);
-            }
-            __nv_bfloat162 bb = __floats2bfloat162_rn(d0, d1);
-            w[j >> 1] = *reinterpret_cast<uint32_t*>(&bb);
-          }
-          *reinterpret_cast<uint4*>(mat + mat_off(r, j0)) = make_uint4(w[0], w[1], w[2], w[3]);
-          *reinterpret_cast<uint4*>(mat + mat_off(r, j0 + 8)) = make_uint4(w[4], w[5], w[6], w[7]);
-        }
-      } else {
-        // rows = keys (token tok), columns = queries i: S^T and dPd^T
-        for (int j0 = 0; j0 < ncols; j0 += 16) {
-          float sv[16], gv[16];
-          tc::tmem_ld16(tmem + lane_addr + kAcc1 + j0, sv);
-          tc::tmem_ld16(tmem + lane_addr + kAcc2 + j0, gv);
-          uint32_t w[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            float o[2] = {0.f, 0.f};
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int i = j0 + j + e;                  // query token
-              if (i < T) {
-                const float pr = exp2f(sv[j + e] * sl2 - stat_a[i]);
-                const float ds = p.p_drop > 0.f ? drop_scale(seed_lo, seed_hi, (uint32_t)(((int64_t)bh * T + i) * T + tok), p.p_drop, keep) : 1.f;
-                o[e] = round == 0 ? pr * ds : p.scale * pr * (gv[j + e] * ds - stat_b[i]);
-              }
-            }
-            __nv_bfloat162 bb = __floats2bfloat162_rn(o[0], o[1]);
-            w[j >> 1] = *reinterpret_cast<uint32_t*>(&bb);
-          }
-          *reinterpret_cast<uint4*>(mat + mat_off(r, j0)) = make_uint4(w[0], w[1], w[2], w[3]);
-          *reinterpret_cast<uint4*>(mat + mat_off(r, j0 + 8)) = make_uint4(w[4], w[5], w[6], w[7]);
-        }
-      }
-      tc::fence_before_sync();
-    } else {
-      // Z buffer 0 = head-dimension columns [0, 128) as two 64-wide chunks of kRowsY token rows (MN-major B operand)
+    auto stage_z = [&](int ps) {                         // head-dimension columns [128 ps, 128 ps + 128) as two 64-wide chunks
+      uint8_t* zb = smem + (ps & 1) * kZBuf;
       for (int q = 0; q < 2; ++q) {
-        const int cv = max(0, min(64, hs - q * 64));
-        if (cv > 0) stage_any(smem + q * kYBytes, zsrc, z_bf16, zld, tok0, T, kRowsY, zcol + q * 64, cv, tid - 128, 128);
+        const int cv = max(0, min(64, hs - ps * 128 - q * 64));
+        if (cv > 0) stage_any(zb + q * kYBytes, z.src, z.bf16, z.ld, tok0, T, kRowsY, z.col + ps * 128 + q * 64, cv, tid, kThreads);
       }
-      cp_async_wait_all();
-    }
-    fence_async_smem();
+    };
+    __syncthreads();                                     // the element-wise stage is complete; the stages / Z buffers are free
+    stage_z(0);
+    cp_async_wait_all();
+    tc::fence_async_smem();
     __syncthreads();
-
     for (int ps = 0; ps < npass; ++ps) {
-      uint8_t* zb = smem + (ps % 3) * kZBuf;
-      const int dvalid = min(128, hs - ps * 128);         // head-dimension columns of this pass
-      const int nmma = dvalid > 64 ? 128 : 64;
-      if (tid == 0) {
-        tc::fence_after_sync();
-        const uint32_t idesc = tc::make_idesc(1u, 0u, 1u, kRowsX, (uint32_t)nmma);
-        const uint32_t sm = tc::smem_u32(mat), sz = tc::smem_u32(zb);
-        const int ksteps = ncols / 16;
-        for (int k = 0; k < ksteps; ++k)
-          tc::umma_f16(tmem + kOut, tc::make_smem_desc(sm + (k >> 2) * kXBytes + (k & 3) * 32, 16, 1024),
-                       tc::make_smem_desc(sz + k * 2048, kYBytes, 1024), idesc, k > 0 ? 1u : 0u);
-        tc::umma_commit(&bars[2]);
-      }
-      if (ps + 1 < npass) {                               // prefetch the next pass's Z while the tensor core works
-        uint8_t* zn = smem + ((ps + 1) % 3) * kZBuf;
-        for (int q = 0; q < 2; ++q) {
-          const int cv = max(0, min(64, hs - (ps + 1) * 128 - q * 64));
-          if (cv > 0) stage_any(zn + q * kYBytes, zsrc, z_bf16, zld, tok0, T, kRowsY, zcol + (ps + 1) * 128 + q * 64, cv, tid, kThreads);
-        }
+      if (ps + 1 < npass) stage_z(ps + 1);               // the other Z buffer (its last pass retired before the barrier below)
+      const int dvalid = min(128, hs - ps * 128);        // head-dimension columns of this pass
+      float* o32 = p.out32_a ? p.out32_a + ps * 128 : nullptr;
+      __nv_bfloat16* o16 = p.out16_a ? p.out16_a + ps * 128 : nullptr;
+      if (dvalid > 64) value_product<128>(mat, smem + (ps & 1) * kZBuf, ncols, wg, t128, row_ok, orow, mul, dvalid, o32, o16);
+      else             value_product<64>(mat, smem + (ps & 1) * kZBuf, ncols, wg, t128, row_ok, orow, mul, dvalid, o32, o16);
+      if (ps + 1 < npass) {
         cp_async_wait_all();
-        fence_async_smem();
+        tc::fence_async_smem();
+        __syncthreads();
       }
-      tc::mbar_wait(&bars[2], ph_out); ph_out ^= 1u;
-      tc::fence_after_sync();
-      if (warp < 4) {
-        const float mul = mode == MODE_FWD ? inv_sum : 1.f;
-        float* o32 = p.out32_a ? p.out32_a + (tok0 + tok) * old + ocol + ps * 128 : nullptr;
-        __nv_bfloat16* o16 = p.out16_a ? p.out16_a + (tok0 + tok) * old + ocol + ps * 128 : nullptr;
-        for (int d0 = 0; d0 < dvalid; d0 += 16) {
-          float v[16];
-          tc::tmem_ld16(tmem + lane_addr + kOut + d0, v);
-          if (row_ok) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 2) {
-              if (d0 + j < dvalid) {                      // (dvalid is even)
-                const float a = v[j] * mul, bq = v[j + 1] * mul;
-                if (o32) *reinterpret_cast<float2*>(o32 + d0 + j) = make_float2(a, bq);
-                if (o16) *reinterpret_cast<__nv_bfloat162*>(o16 + d0 + j) = __floats2bfloat162_rn(a, bq);
-              }
-            }
-          }
-        }
-        tc::fence_before_sync();
-      }
-      __syncthreads();
     }
-  }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem, 512);
   }
 }
 

@@ -1,5 +1,5 @@
 // LiDAR point cloud -> 2-bin BEV histogram (2,256,256), bit-exact with the reference's numpy path
-// (/root/reference/team_code_transfuser/data.py:446-470, `lidar_to_histogram_features`).
+// (team_code_transfuser/data.py:446-470, `lidar_to_histogram_features`).
 //
 // Semantics restated (np.histogramdd with explicit edges = searchsorted(side='right') + last-edge rule):
 //   x edges = -16 + k/8, y edges = -32 + k/8 (k = 0..256; all exactly representable),

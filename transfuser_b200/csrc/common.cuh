@@ -1,4 +1,4 @@
-// Shared helpers for the transfuser_b200 sm_100a kernels.
+// Shared helpers for the transfuser_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -26,12 +26,22 @@ static inline int tfb_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// Per-stream scratch of the fixed-order reductions across CTAs: `floats` fp32 values and `counters` unsigned ints. Counters are
+// ZERO on entry: every kernel that takes a ticket resets it before it returns. The buffers persist and are shared by all launches
+// on the stream (they run one after another); they only grow, and a grown-out buffer is kept, because a captured CUDA graph goes on
+// using the address it was captured with. Defined in api.cu.
+struct TfbScratch {
+  float* f = nullptr;
+  unsigned int* cnt = nullptr;
+};
+int tfb_scratch(TfbScratch& w, size_t floats, size_t counters, cudaStream_t s);
 
 // Grid for a grid-stride elementwise kernel: enough CTAs to fill the chip a few times, never more than needed.
 static inline int tfb_grid(int64_t n, int threads, int waves = 8) {
@@ -84,6 +94,51 @@ __device__ __forceinline__ void tfb_store_bf16x4(__nv_bfloat16* dst, int64_t i4,
   o.x = *reinterpret_cast<uint32_t*>(&lo);
   o.y = *reinterpret_cast<uint32_t*>(&hi);
   reinterpret_cast<uint2*>(dst)[i4] = o;
+}
+
+// Cross-block sums that give the same bits on every run. Every output index i in [0, n_out) gets exactly one contribution from
+// each split s in [0, nsplit) (ordered_store); the last block of the grid to finish (ordered_finish, called by every thread of
+// every block) adds, for each i, the contributions in split order to out[i]. part / cnt: nsplit * n_out floats and one counter
+// of the stream's scratch (TfbScratch).
+struct OrderedSum {
+  float* part;
+  unsigned int* cnt;
+  int nsplit;
+  int64_t n_out;
+};
+static __device__ __forceinline__ void ordered_store(const OrderedSum& o, int split, int64_t i, float v) { o.part[(int64_t)split * o.n_out + i] = v; }
+static __device__ __forceinline__ void ordered_finish(const OrderedSum& o, float* out) {
+  if (!o.cnt) return;                 // summed by ordered_sum_kernel after the launch instead (large n_out)
+  __shared__ bool last;
+  __threadfence();
+  __syncthreads();
+  const int tid = (threadIdx.z * blockDim.y + threadIdx.y) * blockDim.x + threadIdx.x, nthr = blockDim.x * blockDim.y * blockDim.z;
+  if (tid == 0) last = atomicAdd(o.cnt, 1u) == gridDim.x * gridDim.y * gridDim.z - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  for (int64_t i = tid; i < o.n_out; i += nthr) {
+    float s = 0.f;
+    for (int k = 0; k < o.nsplit; ++k) s += __ldcg(o.part + (int64_t)k * o.n_out + i);
+    out[i] += s;
+  }
+  if (tid == 0) *o.cnt = 0u;
+}
+// out[i] += sum over splits k (in order) of part[k][i], one thread per output: the last step of an OrderedSum whose n_out is too
+// large for one CTA (launched after the kernel that stored the partials, with o.cnt = nullptr there).
+static __global__ void __launch_bounds__(256) ordered_sum_kernel(const float* __restrict__ part, int nsplit, int64_t n_out, float* __restrict__ out) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_out; i += (int64_t)gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int k = 0; k < nsplit; ++k) s += part[(int64_t)k * n_out + i];
+    out[i] += s;
+  }
+}
+
+static inline int ordered_alloc(OrderedSum& o, int nsplit, int64_t n_out, cudaStream_t s) {
+  TfbScratch w;
+  const int rc = tfb_scratch(w, (size_t)nsplit * n_out, 1, s);
+  o.part = w.f; o.cnt = w.cnt; o.nsplit = nsplit; o.n_out = n_out;
+  return rc;
 }
 
 // Counter-based RNG for dropout: one 32-bit hash per (seed, element index); regenerated in backward, no mask storage.

@@ -143,11 +143,12 @@ conv_dgrad_kernel(const float* __restrict__ dy, const float* __restrict__ w, flo
 // ---------------------------------------------------------------- wgrad
 // CTA = (pixel range, 32-wide co block x 32-wide ci block of one group); 16x16 threads, each owning a 2x2 (co,ci) patch for
 // all taps. Output pixels are staged 32 at a time: dy rows and the tap-shifted x rows go through smem, partial sums leave
-// the CTA with one atomicAdd per weight (dw must be zeroed by the caller; dbias likewise).
+// the CTA with one partial per weight, the pixel splits added in split order (OrderedSum; dw / dbias zeroed by the launcher).
 template <int KS>
 __global__ void __launch_bounds__(256)
 conv_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dw, float* __restrict__ dbias,
-                  int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int stride, int groups, int pix_per_cta) {
+                  int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int stride, int groups, int pix_per_cta, OrderedSum osw,
+                  OrderedSum osb) {
   constexpr int T = KS * KS, P = KS / 2, PB = 32, CB = 32;
   __shared__ __align__(16) float sdy[PB][CB + 2];
   __shared__ __align__(16) float sx[T][PB][CB + 2];
@@ -216,22 +217,25 @@ conv_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy, flo
 #pragma unroll
       for (int b = 0; b < 2; ++b) {
         int co = co0 + ty * 2 + a, ci = ci0 + tx * 2 + b;
-        if (co < Cog && ci < Cig) atomicAdd(&dw[((int64_t)(g * Cog + co) * Cig + ci) * T + t], acc[t][a * 2 + b]);
+        if (co < Cog && ci < Cig) ordered_store(osw, blockIdx.x, ((int64_t)(g * Cog + co) * Cig + ci) * T + t, acc[t][a * 2 + b]);
       }
     }
   }
-  if (dbias && ib == 0 && threadIdx.x < CB && co0 + threadIdx.x < Cog) atomicAdd(&dbias[g * Cog + co0 + threadIdx.x], bsum);
+  if (dbias && ib == 0 && threadIdx.x < CB && co0 + threadIdx.x < Cog) ordered_store(osb, blockIdx.x, g * Cog + co0 + threadIdx.x, bsum);
+  ordered_finish(osw, dw);
+  if (dbias) ordered_finish(osb, dbias);
 }
 
 // ---------------------------------------------------------------- wgrad, few input channels (the two stems: Cin = 3)
 // The generic kernel above tiles 32 ci x 32 co per CTA: with 3 input channels 29/32 of its lanes and of its smem staging are padding
 // (0.5 TFLOP/s measured on the 160x704 stem). Here a WARP owns one output pixel at a time and its 32 lanes own 32 output channels:
 // dy[p][co] is one coalesced 128-byte load, the <= 4 x KS*KS tap-shifted inputs are warp-uniform (broadcast) loads, and every lane keeps
-// its [ci][tap] accumulators in registers. The 8 warps of a CTA meet in shared memory; one atomicAdd per weight and CTA.
+// its [ci][tap] accumulators in registers. The 8 warps of a CTA meet in shared memory; one partial per weight and CTA (OrderedSum).
 template <int KS>
 __global__ void __launch_bounds__(256)
 conv_wgrad_smallcin_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dw, float* __restrict__ dbias,
-                           int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int stride, int pix_per_cta) {
+                           int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int stride, int pix_per_cta, OrderedSum osw,
+                           OrderedSum osb) {
   constexpr int T = KS * KS, P = KS / 2, CI = 4, NW = 8;
   __shared__ float red[NW][32][CI * T + 1];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -275,22 +279,24 @@ conv_wgrad_smallcin_kernel(const float* __restrict__ x, const float* __restrict_
 #pragma unroll
     for (int w8 = 0; w8 < NW; ++w8) s += red[w8][l][k];
     if (k == CI * T) {
-      if (dbias) atomicAdd(&dbias[oc], s);
+      if (dbias) ordered_store(osb, blockIdx.x, oc, s);
     } else {
       const int c = k / T, t = k % T;
-      if (c < Cin) atomicAdd(&dw[((int64_t)oc * Cin + c) * T + t], s);
+      if (c < Cin) ordered_store(osw, blockIdx.x, ((int64_t)oc * Cin + c) * T + t, s);
     }
   }
+  ordered_finish(osw, dw);
+  if (dbias) ordered_finish(osb, dbias);
 }
 
 // ---------------------------------------------------------------- wgrad of a 1x1 conv with few OUTPUT channels (CenterNet head
 // outputs: 64 -> {1, 2, 3, 12}). dW[co][ci] = sum_p dy[p][co] x[p][ci]: the generic 32 x 32 tile wastes up to 31/32 of its lanes
 // (0.09 TFLOP/s measured for Cout = 1). Here 64 consecutive threads own 64 input channels (x[p][ci..] is one coalesced 256-byte
 // load), the <= 16 dy values of the pixel are block-uniform (broadcast) loads, each thread keeps its [co] accumulators in registers;
-// the 4 pixel phases of a CTA meet in shared memory, one atomicAdd per weight and CTA.
+// the 4 pixel phases of a CTA meet in shared memory, one partial per weight and CTA (OrderedSum).
 __global__ void __launch_bounds__(256)
 conv1x1_wgrad_narrowout_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dw,
-                               float* __restrict__ dbias, int64_t npix, int Cin, int Cout, int pix_per_cta) {
+                               float* __restrict__ dbias, int64_t npix, int Cin, int Cout, int pix_per_cta, OrderedSum osw, OrderedSum osb) {
   constexpr int CO = 16, CB = 64, NP = 4;
   __shared__ float red[NP][CB][CO + 1];
   const int cl = threadIdx.x % CB, ph = threadIdx.x / CB;
@@ -318,7 +324,7 @@ conv1x1_wgrad_narrowout_kernel(const float* __restrict__ x, const float* __restr
     float s = 0.f;
 #pragma unroll
     for (int j = 0; j < NP; ++j) s += red[j][l][c];
-    atomicAdd(&dw[(int64_t)c * Cin + cc], s);
+    ordered_store(osw, blockIdx.x, (int64_t)c * Cin + cc, s);
   }
   if (dbias && blockIdx.y == 0) {                        // dbias[co] = sum_p dy[p][co]: the CTA's pixel range, 16 threads x strided pixels
     __syncthreads();
@@ -334,9 +340,11 @@ conv1x1_wgrad_narrowout_kernel(const float* __restrict__ x, const float* __restr
     if (threadIdx.x < Cout) {
       float s = 0.f;
       for (int q = 0; q < 16; ++q) s += bs[q * CO + threadIdx.x];
-      atomicAdd(&dbias[threadIdx.x], s);
+      ordered_store(osb, blockIdx.x, threadIdx.x, s);
     }
   }
+  ordered_finish(osw, dw);
+  if (dbias) ordered_finish(osb, dbias);
 }
 
 template <int KS>
@@ -387,6 +395,25 @@ int launch_wgrad(const float* x, const float* dy, float* dw, float* dbias, int N
   splits = ceil_div64(npix, ppc);
   if (cudaMemsetAsync(dw, 0, (size_t)Cout * Cig * KS * KS * sizeof(float), stream) != cudaSuccess) return TFB_ERR_DRIVER;
   if (dbias && cudaMemsetAsync(dbias, 0, (size_t)Cout * sizeof(float), stream) != cudaSuccess) return TFB_ERR_DRIVER;
+  // the pixel splits' partial weight / bias gradients, added in split order (the same bits every run)
+  TfbScratch wk;
+  OrderedSum osw, osb;
+  auto partials = [&](int64_t nsplit) -> int {
+    const int64_t ndw = (int64_t)Cout * Cig * KS * KS;
+    const int rc = tfb_scratch(wk, (size_t)(nsplit * (ndw + Cout)), 2, stream);
+    // weight gradients larger than one CTA's share are summed by a grid-wide ordered_sum_kernel after the launch
+    osw = OrderedSum{wk.f, ndw > 16384 ? nullptr : wk.cnt, (int)nsplit, ndw};
+    osb = OrderedSum{wk.f + nsplit * ndw, wk.cnt + 1, (int)nsplit, Cout};
+    return rc;
+  };
+  auto finish = [&]() -> int {
+    TFB_CHECK_LAUNCH();
+    if (!osw.cnt) {
+      ordered_sum_kernel<<<tfb_grid(osw.n_out, 256), 256, 0, stream>>>(osw.part, osw.nsplit, osw.n_out, dw);
+      TFB_CHECK_LAUNCH();
+    }
+    return TFB_OK;
+  };
   if (groups == 1 && KS == 1 && stride == 1 && Cout <= 16) {
     // narrow-output 1x1 conv (head outputs): threads over input channels, dy broadcast (see conv1x1_wgrad_narrowout_kernel)
     const int cib64 = (Cin + 63) / 64;
@@ -395,9 +422,10 @@ int launch_wgrad(const float* x, const float* dy, float* dw, float* dbias, int N
     if (pp < 128) pp = 128;
     pp = ceil_div64(pp, 16) * 16;
     dim3 grid2((unsigned)ceil_div64(npix, pp), cib64);
-    conv1x1_wgrad_narrowout_kernel<<<grid2, 256, 0, stream>>>(x, dy, dw, dbias, npix, Cin, Cout, (int)pp);
-    TFB_CHECK_LAUNCH();
-    return TFB_OK;
+    const int rc = partials(grid2.x);
+    if (rc != TFB_OK) return rc;
+    conv1x1_wgrad_narrowout_kernel<<<grid2, 256, 0, stream>>>(x, dy, dw, dbias, npix, Cin, Cout, (int)pp, osw, osb);
+    return finish();
   }
   if (groups == 1 && Cin <= 4 && KS == 3) {
     // stems: one warp per pixel, lanes over output channels (see conv_wgrad_smallcin_kernel); ~4 waves of CTAs, >= 256 pixels each
@@ -407,14 +435,16 @@ int launch_wgrad(const float* x, const float* dy, float* dw, float* dbias, int N
     if (pp < 256) pp = 256;
     pp = ceil_div64(pp, 8) * 8;
     dim3 grid2((unsigned)ceil_div64(npix, pp), cob32);
-    conv_wgrad_smallcin_kernel<KS><<<grid2, 256, 0, stream>>>(x, dy, dw, dbias, N, H, W, Cin, Ho, Wo, Cout, stride, (int)pp);
-    TFB_CHECK_LAUNCH();
-    return TFB_OK;
+    const int rc = partials(grid2.x);
+    if (rc != TFB_OK) return rc;
+    conv_wgrad_smallcin_kernel<KS><<<grid2, 256, 0, stream>>>(x, dy, dw, dbias, N, H, W, Cin, Ho, Wo, Cout, stride, (int)pp, osw, osb);
+    return finish();
   }
   dim3 grid((unsigned)splits, by);
-  conv_wgrad_kernel<KS><<<grid, 256, 0, stream>>>(x, dy, dw, dbias, N, H, W, Cin, Ho, Wo, Cout, stride, groups, (int)ppc);
-  TFB_CHECK_LAUNCH();
-  return TFB_OK;
+  const int rc = partials(grid.x);
+  if (rc != TFB_OK) return rc;
+  conv_wgrad_kernel<KS><<<grid, 256, 0, stream>>>(x, dy, dw, dbias, N, H, W, Cin, Ho, Wo, Cout, stride, groups, (int)ppc, osw, osb);
+  return finish();
 }
 
 bool conv_args_ok(int N, int H, int W, int Cin, int Cout, int ksize, int stride, int groups) {

@@ -1,11 +1,11 @@
-// Implicit-GEMM 3x3 convolution (stride 1, pad 1, NHWC) on the tcgen05 tensor cores — no im2col buffer.
-// One CTA = one 8x16 spatial tile (128 output pixels = the UMMA M dimension) of one image x one block of output channels.
+// Implicit-GEMM 3x3 convolution (stride 1, pad 1, NHWC) on the wgmma tensor cores — no im2col buffer.
+// One CTA = one 8x16 spatial tile (128 output pixels = two wgmma M = 64 halves) of one image x one block of output channels.
 // For each of the 9 taps and each input-channel chunk, TMA loads the tap-SHIFTED activation patch straight from the NHWC
 // bf16 tensor with a 4-D tensor map (box {KC channels, 16 w, 8 h, 1 n}; halo / image-border pixels are TMA out-of-bounds
 // zero fill = the conv's zero padding) into 128B/64B-swizzled shared memory, where it is already a K-major A operand;
 // the packed weights (K-major B operand, bf16, zero-padded, block-diagonal for grouped convs) come through a 2-D map.
-// All taps / chunks accumulate into ONE fp32 TMEM accumulator; the epilogue adds bias / ReLU and writes fp32 NHWC.
-// dgrad (stride 1) is the same kernel on dy with tap-flipped, transposed packed weights.
+// All taps / chunks accumulate into ONE fp32 register accumulator per consumer warpgroup; the epilogue adds bias / ReLU and
+// writes fp32 NHWC. dgrad (stride 1) is the same kernel on dy with tap-flipped, transposed packed weights.
 // Grouped RegNetY convs (group width 24): two groups share one CTA (N = 48 output channels, 64-channel K window).
 // Replaces cuDNN behind the grouped 3x3 of timm's RegNetY blocks (transfuser.py:145-184) and the dense 3x3 of the
 // decoders / heads (transfuser.py:214-281; model.py:93-99, 581-585). Warp roles as in gemm_tc.cu.
@@ -16,56 +16,39 @@
 namespace {
 
 constexpr int TH = 8, TW = 16, BM = TH * TW;
-
-__device__ __forceinline__ uint64_t smem_desc_kmajor(uint32_t addr, int row_bytes) {
-  // K-major operand, rows of `row_bytes` (128 -> SWIZZLE_128B, 64 -> SWIZZLE_64B); 8-row groups are row_bytes*8 apart.
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;                                    // LBO (ignored for swizzled K-major)
-  d |= (uint64_t)(((uint32_t)row_bytes * 8) >> 4) << 32;     // SBO
-  d |= (uint64_t)1 << 46;                                    // descriptor version (Blackwell)
-  d |= (uint64_t)(row_bytes == 128 ? 2 : 4) << 61;           // SWIZZLE_128B / SWIZZLE_64B
-  return d;
-}
+constexpr int kThreads = 288;                   // warps 0-7: two consumer warpgroups (tile rows 0-3 / 4-7); warp 8: TMA producer
+constexpr int kStageFloats = 16 * 36;           // one warp's epilogue staging block
 
 template <int KC, int NB, int STAGES>
-__global__ void __launch_bounds__(192)
+__global__ void __launch_bounds__(kThreads, NB <= 64 ? 2 : 1)
 conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constant__ CUtensorMap tma_w, float* __restrict__ y,
                   const float* __restrict__ bias, int H, int W, int Cout, int tiles_w, int tiles_h, int c_step, int nchunks,
-                  int nb_real, int relu, int gblocks, int total_tiles, int stride, double* __restrict__ stats) {
+                  int nb_real, int relu, int gblocks, int total_tiles, int stride, double* __restrict__ stats, float* __restrict__ ws,
+                  unsigned int* __restrict__ ws_cnt) {
   // H, W: OUTPUT height / width. stride 2: the activation map steps two pixels per box element, so tile pixel (h, w) reads the
   // input pixel (2h + dy, 2w + dx) of tap (dy, dx).
   // PERSISTENT: tile t = (spatial tile, channel block), channel block fastest (CTAs running together re-use the same activation
-  // patch out of L2); double-buffered TMEM accumulator so the epilogue of tile i overlaps the MMAs of tile i+1.
-  constexpr int ROWB = KC * 2;                 // bytes per smem row
+  // patch out of L2); the producer loads the next tile's stages while the consumers run the epilogue.
+  constexpr int ROWB = KC * 2;                 // bytes per smem row (= swizzle width)
   constexpr int A_BYTES = BM * ROWB, B_BYTES = NB * ROWB, STAGE = A_BYTES + B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
   float* stage_out = reinterpret_cast<float*>(smem + STAGES * STAGE + 256);
-  float* s_stat = stage_out + 4 * 32 * 36;      // [2][Cout] per-channel statistics accumulators (present only when stats != nullptr)
+  float* s_stat = stage_out + 8 * kStageFloats; // [2][Cout] per-channel statistics accumulators (present only when stats != nullptr)
+  float* wstat = s_stat + 2 * Cout;             // [8 warps][2][kStatW] per-tile statistics of each consumer warp (likewise)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int iters = nchunks * 9;
-  constexpr uint32_t kAccCols = NB <= 32 ? 32 : NB <= 64 ? 64 : 128;
-  constexpr uint32_t kTmemCols = 2 * kAccCols;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tma_x);
     tc::tma_prefetch_desc(&tma_w);
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { tc::mbar_init(&tmem_full_bar[s], 1); tc::mbar_init(&tmem_empty_bar[s], 4); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 8); }   // 8 consumer warps
     tc::mbar_fence_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, kTmemCols);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto decode = [&](int t, int& gb, int& n, int& h0, int& w0) {
     gb = t % gblocks;
@@ -75,7 +58,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_consta
     n = sp; h0 = th * TH; w0 = tw * TW;
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int it = 0;
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
@@ -92,90 +75,75 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::make_idesc(1u, 0u, 0u, BM, NB);  // bf16 x bf16 -> fp32, both K-major
-      int it = 0, lt = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
-        const int as = lt & 1, aph = (lt >> 1) & 1;
-        tc::mbar_wait(&tmem_empty_bar[as], aph ^ 1);
-        tc::fence_after_sync();
-        const uint32_t acc_addr = tmem_base + (uint32_t)as * kAccCols;
-        for (int i = 0; i < iters; ++i, ++it) {
-          const int s = it % STAGES, ph = (it / STAGES) & 1;
-          tc::mbar_wait(&full_bar[s], ph);
-          tc::fence_after_sync();
-          const uint32_t sa = tc::smem_u32(smem + s * STAGE), sb = sa + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < KC / 16; ++k)
-            tc::umma_f16(acc_addr, smem_desc_kmajor(sa + k * 32, ROWB), smem_desc_kmajor(sb + k * 32, ROWB), idesc, (i > 0 || k > 0) ? 1u : 0u);
-          tc::umma_commit(&empty_bar[s]);
-        }
-        tc::umma_commit(&tmem_full_bar[as]);
-      }
-    }
   } else {
-    const int q = warp & 3;
-    float* stage = stage_out + q * (32 * 36);
-    int lt = 0;
-    if (stats) tc::stat_clear(s_stat, Cout, (int)threadIdx.x - 64);
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
+    const int wg = warp >> 2, wq = warp & 3;
+    float* stage = stage_out + warp * kStageFloats;
+    float acc[NB / 2];
+    int it = 0;
+    if (stats) tc::stat_clear(s_stat, Cout, (int)threadIdx.x);
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int gb, n, h0, w0;
       decode(t, gb, n, h0, w0);
-      const int as = lt & 1, aph = (lt >> 1) & 1;
-      tc::mbar_wait(&tmem_full_bar[as], aph);
-      tc::fence_after_sync();
-      const uint32_t acc_addr = tmem_base + (uint32_t)as * kAccCols + ((uint32_t)(q * 32) << 16);
+      int prev = 0;
+      for (int i = 0; i < iters; ++i, ++it) {
+        const int s = it % STAGES, ph = (it / STAGES) & 1;
+        tc::mbar_wait(&full_bar[s], ph);
+        const uint32_t sa = tc::smem_u32(smem + s * STAGE) + wg * 64 * ROWB, sb = tc::smem_u32(smem + s * STAGE) + A_BYTES;
+        tc::fence_acc(acc);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < KC / 16; ++k)
+          tc::wgmma_bf16<0, 0>(acc, tc::make_smem_desc(sa + k * 32, 16, ROWB * 8, ROWB), tc::make_smem_desc(sb + k * 32, 16, ROWB * 8, ROWB),
+                               (i > 0 || k > 0) ? 1u : 0u);
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        tc::fence_acc(acc);
+        if (i > 0) { __syncwarp(); if (lane == 0) tc::mbar_arrive(&empty_bar[prev]); }
+        prev = s;
+      }
+      tc::wgmma_wait<0>();
+      tc::fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+
+      // this warp's 16 accumulator rows = tile row 4 * wg + wq = output pixels (h0 + 4 * wg + wq, w0 + 0..15)  (W fastest in the TMA box)
+      const int h = h0 + wg * 4 + wq;
       const int nvalid = min(nb_real, Cout - gb * nb_real);
       float* ytile = y + (int64_t)gb * nb_real;
       const float* bp = bias ? bias + gb * nb_real : nullptr;
       const bool fast = (Cout & 3) == 0 && ((gb * nb_real) & 3) == 0 && ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
       if (fast) {
-        // accumulator row r of this warp's band = pixel (h0 + (q*32 + r) / 16, w0 + (q*32 + r) % 16)  (W fastest in the TMA box)
-#pragma unroll 1
-        for (int c0 = 0; c0 < NB; c0 += 32) {
-          const int cols_valid = nvalid - c0;
-          if (cols_valid <= 0) break;
-          tc::epilogue_chunk32(acc_addr + (uint32_t)c0, stage,
-                               [=](int row) -> int64_t {
-                                 const int r = q * 32 + row, h = h0 + r / TW, w = w0 + r % TW;
-                                 return (h < H && w < W) ? (((int64_t)n * H + h) * W + w) * Cout + c0 : (int64_t)-1;
-                               },
-                               cols_valid, bp ? bp + c0 : nullptr, 1.f, relu, lane, ytile, nullptr,
-                               stats ? s_stat + gb * nb_real + c0 : nullptr, stats ? s_stat + Cout + gb * nb_real + c0 : nullptr);
-        }
-      } else {
-        const int r = q * 32 + lane;
-        const int h = h0 + r / TW, w = w0 + r % TW;
-        const bool pix_ok = h < H && w < W;
-        float* yp = ytile + (((int64_t)n * H + h) * W + w) * Cout;
-#pragma unroll 1
-        for (int c0 = 0; c0 < NB; c0 += 16) {
-          float v[16];
-          tc::tmem_ld16(acc_addr + (uint32_t)c0, v);
-          if (pix_ok) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              if (c0 + j < nvalid) {
-                float o = v[j] + (bp ? bp[c0 + j] : 0.f);
-                if (relu) o = fmaxf(o, 0.f);
-                yp[c0 + j] = o;
-              }
-            }
+        for (int c = 0; c < (NB + 31) / 32; ++c) {
+          const int c0 = c * 32;
+          const int cols_valid = min(nvalid - c0, NB - c0);
+          if (cols_valid <= 0) break;
+          tc::frag_to_stage(stage, acc, c, lane);
+          tc::stage_to_global(stage,
+                              [=](int row) -> int64_t {
+                                const int w = w0 + row;
+                                return (h < H && w < W) ? (((int64_t)n * H + h) * W + w) * Cout + c0 : (int64_t)-1;
+                              },
+                              cols_valid, bp ? bp + c0 : nullptr, 1.f, relu, lane, ytile, nullptr,
+                              stats ? wstat + (warp * 2) * tc::kStatW + c0 : nullptr,
+                              stats ? wstat + (warp * 2 + 1) * tc::kStatW + c0 : nullptr);
+        }
+        if (stats) tc::stat_fold(s_stat, wstat, Cout, gb * nb_real, nvalid, (int)threadIdx.x);
+      } else {
+        const int t128 = threadIdx.x & 127;
+#pragma unroll
+        for (int i = 0; i < NB / 2; ++i) {
+          const int r = tc::frag_row(t128, i) - wq * 16, col = tc::frag_col(t128, i);   // r: row inside this warp's band
+          const int w = w0 + r;
+          if (h < H && w < W && col < nvalid) {
+            float o = acc[i] + (bp ? bp[col] : 0.f);
+            if (relu) o = fmaxf(o, 0.f);
+            ytile[(((int64_t)n * H + h) * W + w) * Cout + col] = o;
           }
         }
       }
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tmem_empty_bar[as]);
     }
-    if (stats) tc::stat_flush(s_stat, stats, Cout, (int)threadIdx.x - 64);
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, kTmemCols);
+    if (stats) tc::stat_flush(s_stat, stats, Cout, (int)threadIdx.x, ws, ws_cnt);
   }
 }
 
@@ -185,8 +153,9 @@ int launch_conv(const void* x16, const void* wpack, const float* bias, float* y,
   const int H = (Hin - 1) / stride + 1, W = (Win - 1) / stride + 1;       // output size (kernel 3, pad 1)
   constexpr int STAGES = NB <= 64 ? 6 : 4;
   constexpr int STAGE = BM * KC * 2 + NB * KC * 2;
-  constexpr int SMEM0 = STAGES * STAGE + 256 + 4 * 32 * 36 * 4 + 1024;   // ring + barriers/TMEM slot + epilogue staging + alignment slack
-  const int SMEM = SMEM0 + (stats ? 2 * Cy * (int)sizeof(float) : 0);    // + per-channel statistics accumulators
+  constexpr int SMEM0 = STAGES * STAGE + 256 + 8 * kStageFloats * 4 + 1024;   // ring + barriers + epilogue staging + alignment slack
+  // + per-channel statistics accumulators and the consumer warps' per-tile statistics
+  const int SMEM = SMEM0 + (stats ? (2 * Cy + 8 * 2 * tc::kStatW) * (int)sizeof(float) : 0);
   CUtensorMap mx, mw;
   const uint64_t xd[4] = {(uint64_t)Cx, (uint64_t)Win, (uint64_t)Hin, (uint64_t)N};
   const uint64_t xs[3] = {(uint64_t)Cx * 2, (uint64_t)Win * Cx * 2, (uint64_t)Hin * Win * Cx * 2};
@@ -207,7 +176,7 @@ int launch_conv(const void* x16, const void* wpack, const float* bias, float* y,
   auto kern = conv3x3_tc_kernel<KC, NB, STAGES>;
   static bool attr_done = false;
   if (!attr_done) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM0 + 2 * 2048 * (int)sizeof(float)) != cudaSuccess) return TFB_ERR_DRIVER;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM0 + (2 * 2048 + 8 * 2 * tc::kStatW) * (int)sizeof(float)) != cudaSuccess) return TFB_ERR_DRIVER;
     attr_done = true;
   }
   const int tiles_w = (W + TW - 1) / TW, tiles_h = (H + TH - 1) / TH;
@@ -217,7 +186,13 @@ int launch_conv(const void* x16, const void* wpack, const float* bias, float* y,
   const int per_sm = (SMEM <= 110 * 1024) ? 2 : 1;
   const int64_t cap = (int64_t)tfb_num_sms() * per_sm;
   const int grid = (int)(total < cap ? total : cap);
-  kern<<<grid, 192, SMEM, stream>>>(mx, mw, y, bias, H, W, Cy, tiles_w, tiles_h, c_step, nchunks, nb_real, relu, gblocks, (int)total, stride, stats);
+  TfbScratch wk;                 // the CTAs' statistics, reduced in CTA order by the last one
+  if (stats) {
+    const int rc = tfb_scratch(wk, (size_t)grid * 2 * Cy, 1, stream);
+    if (rc != TFB_OK) return rc;
+  }
+  kern<<<grid, kThreads, SMEM, stream>>>(mx, mw, y, bias, H, W, Cy, tiles_w, tiles_h, c_step, nchunks, nb_real, relu, gblocks, (int)total, stride, stats,
+                                         wk.f, wk.cnt);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }

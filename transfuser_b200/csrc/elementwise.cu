@@ -38,10 +38,11 @@ __global__ void __launch_bounds__(256) act_kernel(const float* __restrict__ y, c
 }
 
 // out[n][c] (+)= scale * sum_p x[n][p][c] (MODE 0)  or  sum_p x[n][p][c] * z[n][p][c] (MODE 1: SE gate gradient)
-// block (32 channel quads, 8 row phases); grid (quad slabs, n, HW splits); partial sums leave through fp32 atomics (out zeroed).
+// block (32 channel quads, 8 row phases); grid (quad slabs, n, HW splits); the splits' partial sums are added in split order
+// (OrderedSum; out zeroed).
 template <int MODE>
 __global__ void __launch_bounds__(256) pool_hw_kernel(const float* __restrict__ x, const float* __restrict__ z, float* __restrict__ out,
-                                                      int HW, int C, float scale) {
+                                                      int HW, int C, float scale, OrderedSum os) {
   __shared__ float4 sm[8][33];
   const int n = blockIdx.y, c = (blockIdx.x * 32 + threadIdx.x) * 4;
   float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -63,9 +64,11 @@ __global__ void __launch_bounds__(256) pool_hw_kernel(const float* __restrict__ 
     float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) { const float4 v = sm[j][threadIdx.x]; t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w; }
-    float* o = out + (int64_t)n * C + c;
-    atomicAdd(o + 0, t.x * scale); atomicAdd(o + 1, t.y * scale); atomicAdd(o + 2, t.z * scale); atomicAdd(o + 3, t.w * scale);
+    const int64_t o = (int64_t)n * C + c;
+    ordered_store(os, blockIdx.z, o + 0, t.x * scale); ordered_store(os, blockIdx.z, o + 1, t.y * scale);
+    ordered_store(os, blockIdx.z, o + 2, t.z * scale); ordered_store(os, blockIdx.z, o + 3, t.w * scale);
   }
+  ordered_finish(os, out);
 }
 
 // pool_hw_kernel for narrow maps (C / 4 <= 128 channel quads): a block covers 256 / C4 whole pixel rows of ONE sample per iteration,
@@ -73,7 +76,7 @@ __global__ void __launch_bounds__(256) pool_hw_kernel(const float* __restrict__ 
 // grid (splits over the pixels, n).
 template <int MODE>
 __global__ void __launch_bounds__(256) pool_hw_flat_kernel(const float* __restrict__ x, const float* __restrict__ z, float* __restrict__ out,
-                                                           int HW, int C, float scale) {
+                                                           int HW, int C, float scale, OrderedSum os) {
   const int C4 = C / 4, RPB = 256 / C4;
   const int t = threadIdx.x, q = t % C4, rr = t / C4, n = blockIdx.y;
   float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -95,9 +98,11 @@ __global__ void __launch_bounds__(256) pool_hw_flat_kernel(const float* __restri
   if (t < C4) {
     float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int j = 0; j < RPB; ++j) { const float4 v = sm[j * C4 + t]; s4.x += v.x; s4.y += v.y; s4.z += v.z; s4.w += v.w; }
-    float* o = out + (int64_t)n * C + t * 4;
-    atomicAdd(o + 0, s4.x * scale); atomicAdd(o + 1, s4.y * scale); atomicAdd(o + 2, s4.z * scale); atomicAdd(o + 3, s4.w * scale);
+    const int64_t o = (int64_t)n * C + t * 4;
+    ordered_store(os, blockIdx.x, o + 0, s4.x * scale); ordered_store(os, blockIdx.x, o + 1, s4.y * scale);
+    ordered_store(os, blockIdx.x, o + 2, s4.z * scale); ordered_store(os, blockIdx.x, o + 3, s4.w * scale);
   }
+  ordered_finish(os, out);
 }
 
 // y[n][p][c] = x[n][p][c] * gate[n][c]  (+ add[n][c] * add_scale); VEC = 4 when C % 4 == 0 (16-byte accesses)
@@ -698,7 +703,8 @@ __global__ void __launch_bounds__(256) se_mlp_bwd1_kernel(const float* __restric
                                                           const float* __restrict__ h, const float* __restrict__ w2,
                                                           float* __restrict__ dw2, float* __restrict__ db2, float* __restrict__ dh_acc,
                                                           int N, int C, int Cr) {
-  // one CTA per 64-channel chunk of C. dh_acc[N][Cr] (ZERO on entry) receives this chunk's share of ds w2 through fp32 atomics.
+  // one CTA per 64-channel chunk of C. dh_acc[chunk][N][Cr] receives this chunk's share of ds w2; se_mlp_bwd2_kernel adds the chunks
+  // in chunk order (the same bits every run).
   __shared__ float ds[SE_MAX_N * SE_CHUNK];  // [N][SE_CHUNK]
   __shared__ float hs[SE_MAX_N * SE_MAX_CR]; // [N][Cr]
   const int c0 = blockIdx.x * SE_CHUNK;
@@ -740,7 +746,7 @@ __global__ void __launch_bounds__(256) se_mlp_bwd1_kernel(const float* __restric
     }
 #pragma unroll
     for (int n = 0; n < SE_MAX_N; ++n)
-      if (n < N) atomicAdd(dh_acc + (int64_t)n * Cr + r, acc[n]);
+      if (n < N) dh_acc[((int64_t)blockIdx.x * N + n) * Cr + r] = acc[n];
   }
 }
 
@@ -753,7 +759,12 @@ __global__ void __launch_bounds__(256) se_mlp_bwd2_kernel(const float* __restric
   __shared__ float red[SE_SLICES - 1][SE_MAX_N][SE_CHUNK];   // slices 1.. (slice 0 keeps its sums in registers): 48 KiB of static smem in total
   const int c0 = blockIdx.x * SE_CHUNK;
   const int cw = min(SE_CHUNK, C - c0);
-  for (int i = threadIdx.x; i < SE_MAX_N * Cr; i += blockDim.x) dh[i] = (i < N * Cr && h[i] > 0.f) ? dh_acc[i] : 0.f;
+  for (int i = threadIdx.x; i < SE_MAX_N * Cr; i += blockDim.x) {
+    float s = 0.f;
+    if (i < N * Cr && h[i] > 0.f)
+      for (int k = 0; k < (int)gridDim.x; ++k) s += dh_acc[(int64_t)k * N * Cr + i];
+    dh[i] = s;
+  }
   for (int i = threadIdx.x; i < N * SE_CHUNK; i += blockDim.x) {
     const int n = i / SE_CHUNK, j = i % SE_CHUNK;
     ps[i] = j < cw ? pooled[(int64_t)n * C + c0 + j] : 0.f;
@@ -847,7 +858,10 @@ TFB_API int tfb_pool_hw_fwd(const float* x, float* out, int N, int HW, int C, cu
   int splits = (HW + 255) / 256;
   if (splits > 32) splits = 32;
   dim3 grid((C / 4 + 31) / 32, N, splits), block(32, 8);
-  pool_hw_kernel<0><<<grid, block, 0, stream>>>(x, nullptr, out, HW, C, 1.f / (float)HW);
+  OrderedSum os;
+  const int rc = ordered_alloc(os, splits, (int64_t)N * C, stream);
+  if (rc != TFB_OK) return rc;
+  pool_hw_kernel<0><<<grid, block, 0, stream>>>(x, nullptr, out, HW, C, 1.f / (float)HW, os);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
@@ -880,27 +894,35 @@ TFB_API int tfb_se_bwd_reduce(const float* x, const float* dy, float* dgate, int
     const int cap = (4 * tfb_num_sms() + N - 1) / N;
     if (sp > cap) sp = cap;
     if (sp < 1) sp = 1;
-    pool_hw_flat_kernel<1><<<dim3(sp, N), 256, 0, stream>>>(x, dy, dgate, HW, C, 1.f);
+    OrderedSum os;
+    const int rc = ordered_alloc(os, sp, (int64_t)N * C, stream);
+    if (rc != TFB_OK) return rc;
+    pool_hw_flat_kernel<1><<<dim3(sp, N), 256, 0, stream>>>(x, dy, dgate, HW, C, 1.f, os);
     TFB_CHECK_LAUNCH();
     return TFB_OK;
   }
-  pool_hw_kernel<1><<<grid, block, 0, stream>>>(x, dy, dgate, HW, C, 1.f);
+  OrderedSum os;
+  const int rc = ordered_alloc(os, splits, (int64_t)N * C, stream);
+  if (rc != TFB_OK) return rc;
+  pool_hw_kernel<1><<<grid, block, 0, stream>>>(x, dy, dgate, HW, C, 1.f, os);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
 // Fused backward of the squeeze-excite MLP (see se_mlp_bwd1_kernel): dgate, gate, pooled [N,C]; h [N,Cr]; w1 [Cr,C]; w2 [C,Cr] ->
 // dw1 [Cr,C], db1 [Cr], dw2 [C,Cr], db2 [C], dpool [N,C] (all overwritten). N <= 16, Cr <= 512.
-// dh_part: workspace of at least N * Cr floats (cleared here: one memset node).
+// dh_part: unused (kept for the C-ABI); the per-chunk partial sums live in a per-launch workspace.
 TFB_API int tfb_se_mlp_bwd(const float* dgate, const float* gate, const float* h, const float* pooled, const float* w1, const float* w2,
                            float* dw1, float* db1, float* dw2, float* db2, float* dpool, float* dh_part, int N, int C, int Cr,
                            cudaStream_t stream) {
   TFB_REQUIRE(dgate && gate && h && pooled && w1 && w2 && dw1 && db1 && dw2 && db2 && dpool && dh_part);
   TFB_REQUIRE(N > 0 && N <= SE_MAX_N && C > 0 && Cr > 0 && Cr <= SE_MAX_CR);
   const int nchunks = (C + SE_CHUNK - 1) / SE_CHUNK;
-  if (cudaMemsetAsync(dh_part, 0, (size_t)N * Cr * sizeof(float), stream) != cudaSuccess) return TFB_ERR_DRIVER;
-  se_mlp_bwd1_kernel<<<nchunks, 256, 0, stream>>>(dgate, gate, h, w2, dw2, db2, dh_part, N, C, Cr);
+  TfbScratch w;
+  const int rc = tfb_scratch(w, (size_t)nchunks * N * Cr, 0, stream);
+  if (rc != TFB_OK) return rc;
+  se_mlp_bwd1_kernel<<<nchunks, 256, 0, stream>>>(dgate, gate, h, w2, dw2, db2, w.f, N, C, Cr);
   TFB_CHECK_LAUNCH();
-  se_mlp_bwd2_kernel<<<nchunks, 256, 0, stream>>>(dh_part, h, pooled, w1, dw1, db1, dpool, N, C, Cr);
+  se_mlp_bwd2_kernel<<<nchunks, 256, 0, stream>>>(w.f, h, pooled, w1, dw1, db1, dpool, N, C, Cr);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }

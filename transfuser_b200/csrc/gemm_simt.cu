@@ -1,8 +1,8 @@
 // fp32 CUDA-core GEMM (exact-fp32 path): C = alpha * op(A) * op(B) + beta * C (+ bias[n]) (ReLU optional),
 // row-major, arbitrary leading dimensions, two-level strided batching (used for per-(sample, head) attention
-// products and for every shape the tcgen05 path does not take: tiny M, odd leading dimensions, parity mode).
+// products and for every shape the tensor-core path does not take: tiny M, odd leading dimensions, parity mode).
 // Replaces the cuBLAS calls behind nn.Linear / 1x1 nn.Conv2d / torch.matmul in the reference
-// (/root/reference/team_code_transfuser/transfuser.py:510-527, 538-543; model.py:592-605).
+// (team_code_transfuser/transfuser.py:510-527, 538-543; model.py:592-605).
 // 128x64x16 tiles, 256 threads, 8x4 outputs per thread, register-prefetched double buffering, 8-byte vector loads when the
 // operand's contiguous dimension allows it (head offsets of the packed q|k|v buffer are only 8-byte aligned).
 #include "common.cuh"

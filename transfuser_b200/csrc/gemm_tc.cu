@@ -1,13 +1,14 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a:  C[M,N] = alpha * op(A)[M,K] * op(B)[K,N] (+ bias[n]) (+ beta*C) (ReLU)
-// Operands fp32 in HBM, fed to the tensor cores as TF32 (kind::tf32, fp32 accumulate in TMEM), or bf16 (kind::f16).
+// wgmma / TMA GEMM for sm_90a:  C[M,N] = alpha * op(A)[M,K] * op(B)[K,N] (+ bias[n]) (+ beta*C) (ReLU)
+// Operands fp32 in HBM, fed to the tensor cores as TF32 (wgmma .tf32, fp32 accumulate in registers), or bf16.
 // All four transpose combinations are served without materialising a transpose: a K-contiguous operand is a
-// "K-major" UMMA operand, an M/N-contiguous operand is an "MN-major" one; both are staged by TMA into
+// "K-major" wgmma operand, an M/N-contiguous operand is an "MN-major" (transposed) one; both are staged by TMA into
 // 128B-swizzled shared memory and described to the MMA by a shared-memory matrix descriptor.
 //   forward  y = x W^T      : A K-major (x[M,K]),  B K-major (W[N,K])
 //   dgrad    dx = dy W      : A K-major (dy[M,N']), B MN-major (W[N',K'] read as [k][n])
 //   wgrad    dW = dy^T x    : A MN-major (dy[M',N] read as [k][m]), B MN-major (x[M',K] read as [k][n]); split-K + atomics
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer (one lane), warps 2-5 = epilogue
-// (TMEM -> registers -> global). One 128 x BN output tile per CTA, STAGES-deep mbarrier ring between TMA and MMA.
+// Warp roles (288 threads): warps 0-7 = two consumer warpgroups (wgmma issue on rows 0-63 / 64-127 of the tile, then the
+// epilogue registers -> global), warp 8 = TMA producer. One 128 x BN output tile at a time per CTA, STAGES-deep mbarrier ring
+// between TMA and the MMAs.
 // Replaces cuBLAS/cuDNN behind nn.Linear and 1x1 nn.Conv2d (transfuser.py:510-527,538-543; timm RegNet 1x1 convs).
 #include <stdlib.h>
 
@@ -32,53 +33,49 @@ template <> struct Elem<__nv_bfloat16> {
   static constexpr CUtensorMapDataType kTmaType = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 };
 
-// Shared memory: STAGES x (A tile 128 x 128 B | B tile BN x 128 B), barriers, 4 x (32 x 36 floats) epilogue staging. BN (the tile
-// width, any multiple of 16 up to 256; a multiple of 64 for an MN-major B) and STAGES are RUNTIME values: the host picks the width
-// that fills whole waves of the persistent grid (M = 1740 token GEMMs: N = 1512 -> 160, N = 4536 -> 224) and the deepest ring that fits.
+// Shared memory: STAGES x (A tile 128 x 128 B | B tile BN x 128 B), barriers, 8 x (16 x 36 floats) epilogue staging. BN (the tile
+// width: a multiple of 32 up to kMaxBN, a multiple of 64 for an MN-major B) is a template parameter because it is the N of the wgmma
+// instruction and the size of the register accumulator; the host picks the width that fills whole waves of the persistent grid
+// and the deepest ring that fits. STAGES is a runtime value. kMaxBN = 192: with 288 threads ptxas budgets 168 registers per thread
+// (warpgroup granularity), and the 224- / 256-wide accumulators (112 / 128 registers) spill around the wgmma.
 int g_max_ctas = 0;                                           // tfb_gemm_set_max_ctas: cap of the persistent grid (0 = one CTA per SM)
+constexpr int kMaxBN = 192;
+constexpr int kThreads = 288;                                 // warps 0-7: two consumer warpgroups; warp 8: TMA producer
+constexpr int kStageFloats = 16 * 36;                         // one warp's epilogue staging block (16 rows, padded stride 36)
 constexpr int kABytes = BM * 128;
-constexpr int kSmemMax = 232448;                              // 227 KB opt-in limit
-constexpr int kSmemFixed = 256 + 4 * 32 * 36 * 4 + 1024;      // barriers + epilogue staging + alignment slack
-constexpr uint32_t kAccCols = 256;                            // TMEM columns per accumulator buffer (2 buffers = all 512)
+constexpr int kSmemMax = 232448 - 64;                         // 227 KB opt-in limit, less the kernel's static shared flags
+constexpr int kSmemFixed = 256 + 8 * kStageFloats * 4 + 1024; // barriers + epilogue staging + alignment slack
 
-template <typename T, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(192, 1)
+template <typename T, bool A_MN, bool B_MN, int BN>
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, float* __restrict__ Cbase,
                int64_t ldc, int M, int N, int num_kb, int kb_per_split, const float* __restrict__ bias, float alpha, float beta,
                int relu, int atomic_out, int splits, int a_step, int b_step, int64_t c_bstride, int tiles_m, int tiles_n,
-               int total_tiles, int BN, int STAGES, double* __restrict__ stats, __nv_bfloat16* __restrict__ C16) {
+               int total_tiles, int STAGES, double* __restrict__ stats, __nv_bfloat16* __restrict__ C16, float* __restrict__ ws,
+               unsigned int* __restrict__ ws_cnt) {
   // PERSISTENT: gridDim.x CTAs (<= one per SM) walk the tile list t = blockIdx.x, += gridDim.x. A tile is (m-tile, n-tile, z),
   // z = batch * splits + split; m fastest so that concurrently running CTAs share the same B (weight) tile in L2.
-  // The TMEM accumulator is double buffered (2 x BN columns): the epilogue warps drain tile i while the MMA warp already
-  // accumulates tile i+1, and the TMA producer runs ahead across tile boundaries through the shared-memory ring.
+  // Consumer warpgroup g (warps 4g..4g+3) owns rows [64g, 64g + 64) of the 128 x BN tile as a wgmma register accumulator;
+  // the TMA producer runs ahead across tile boundaries through the shared-memory ring while the consumers run the epilogue.
   using E = Elem<T>;
   constexpr int BK = E::kPerRow;  // K elements per stage
-  const int stage_bytes = kABytes + BN * 128;
+  constexpr int stage_bytes = kABytes + BN * 128;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;      // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
+  float* stage_out = reinterpret_cast<float*>(smem + STAGES * stage_bytes + 256);
+  float* s_stat = stage_out + 8 * kStageFloats;  // [2][N] per-column statistics accumulators (present only when stats != nullptr)
+  float* wstat = s_stat + 2 * N;                 // [8 warps][2][kStatW] per-tile statistics of each consumer warp (likewise)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t kTmemCols = 2 * kAccCols;
-  float* stage_out = reinterpret_cast<float*>(smem + STAGES * stage_bytes + 256);
-  float* s_stat = stage_out + 4 * 32 * 36;       // [2][N] per-column statistics accumulators (present only when stats != nullptr)
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tma_a);
     tc::tma_prefetch_desc(&tma_b);
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { tc::mbar_init(&tmem_full_bar[s], 1); tc::mbar_init(&tmem_empty_bar[s], 4); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 8); }   // 8 consumer warps
     tc::mbar_fence_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, kTmemCols);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   // decode tile t -> coordinates
   auto decode = [&](int t, int& m0, int& n0, int& bz, int& sz, int& kb_begin, int& nkb) {
@@ -91,12 +88,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     nkb = min(num_kb, kb_begin + kb_per_split) - kb_begin;   // >= 1 by construction
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===== TMA producer =====
     if (lane == 0) {
       int s = 0, ph = 0;
-      const int nb_chunks = (BN + E::kPerRow - 1) / E::kPerRow;
-      const uint32_t tx_bytes = (uint32_t)(kABytes + (B_MN ? nb_chunks * BK * 128 : BN * 128));
+      constexpr int nb_chunks = (BN + E::kPerRow - 1) / E::kPerRow;
+      constexpr uint32_t tx_bytes = (uint32_t)(kABytes + (B_MN ? nb_chunks * BK * 128 : BN * 128));
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         int m0, n0, bz, sz, kb_begin, nkb;
         decode(t, m0, n0, bz, sz, kb_begin, nkb);
@@ -117,6 +114,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           if (!B_MN) {
             tc::tma_load_2d(&tma_b, &full_bar[s], sb, k0, bn0);
           } else {
+#pragma unroll
             for (int j = 0; j < nb_chunks; ++j)
               tc::tma_load_2d(&tma_b, &full_bar[s], sb + j * BK * 128, bn0 + j * E::kPerRow, k0);
           }
@@ -124,107 +122,117 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = tc::make_idesc(E::kFmt, A_MN ? 1u : 0u, B_MN ? 1u : 0u, BM, (uint32_t)BN);
-      int s = 0, ph = 0, lt = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
-        int m0, n0, bz, sz, kb_begin, nkb;
-        decode(t, m0, n0, bz, sz, kb_begin, nkb);
-        const int as = lt & 1, aph = (lt >> 1) & 1;
-        tc::mbar_wait(&tmem_empty_bar[as], aph ^ 1);   // epilogue has drained this accumulator buffer
-        tc::fence_after_sync();
-        const uint32_t acc_addr = tmem_base + (uint32_t)as * kAccCols;
-        for (int i = 0; i < nkb; ++i) {
-          tc::mbar_wait(&full_bar[s], ph);
-          tc::fence_after_sync();
-          const uint32_t sa = tc::smem_u32(smem + s * stage_bytes);
-          const uint32_t sb = sa + kABytes;
-#pragma unroll
-          for (int k = 0; k < BK / E::kUmmaK; ++k) {
-            // K-major: advance 32 B inside the 128 B swizzle row; MN-major: advance kUmmaK rows of 128 B.
-            const uint32_t a_off = A_MN ? k * E::kUmmaK * 128 : k * E::kUmmaK * (int)sizeof(T);
-            const uint32_t b_off = B_MN ? k * E::kUmmaK * 128 : k * E::kUmmaK * (int)sizeof(T);
-            const uint64_t adesc = tc::make_smem_desc(sa + a_off, A_MN ? BK * 128 : 16, 1024);
-            const uint64_t bdesc = tc::make_smem_desc(sb + b_off, B_MN ? BK * 128 : 16, 1024);
-            const uint32_t acc = (i > 0 || k > 0) ? 1u : 0u;
-            if (sizeof(T) == 4) tc::umma_tf32(acc_addr, adesc, bdesc, idesc, acc);
-            else                tc::umma_f16(acc_addr, adesc, bdesc, idesc, acc);
-          }
-          tc::umma_commit(&empty_bar[s]);  // frees the smem slot when these MMAs retire
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        tc::umma_commit(&tmem_full_bar[as]);  // accumulator complete
-      }
-    }
   } else {
-    // ===== epilogue: warps 2..5 own TMEM lane quarters (warp % 4) =====
-    const int q = warp & 3;
-    int lt = 0;
-    if (stats) tc::stat_clear(s_stat, N, (int)threadIdx.x - 64);
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
+    // ===== consumers: wgmma issue + epilogue =====
+    const int wg = warp >> 2, t128 = threadIdx.x & 127;
+    float acc[BN / 2];
+    int s = 0, ph = 0;
+    if (stats) tc::stat_clear(s_stat, N, (int)threadIdx.x);
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int m0, n0, bz, sz, kb_begin, nkb;
       decode(t, m0, n0, bz, sz, kb_begin, nkb);
-      const int as = lt & 1, aph = (lt >> 1) & 1;
-      tc::mbar_wait(&tmem_full_bar[as], aph);
-      tc::fence_after_sync();
-      const int m = m0 + q * 32 + lane;
+      int prev = 0;
+      for (int i = 0; i < nkb; ++i) {
+        tc::mbar_wait(&full_bar[s], ph);
+        const uint32_t base = tc::smem_u32(smem + s * stage_bytes);
+        // this warpgroup's 64 rows: K-major A: 64 rows of 128 B further; MN-major A: the second 64-element M chunk
+        const uint32_t sa = base + (A_MN ? wg * BK * 128 : wg * 64 * 128), sb = base + kABytes;
+        tc::fence_acc(acc);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / E::kUmmaK; ++k) {
+          // K-major: advance 32 B inside the 128 B swizzle row; MN-major: advance kUmmaK rows of 128 B.
+          const uint32_t a_off = A_MN ? k * E::kUmmaK * 128 : k * E::kUmmaK * (int)sizeof(T);
+          const uint32_t b_off = B_MN ? k * E::kUmmaK * 128 : k * E::kUmmaK * (int)sizeof(T);
+          const uint64_t adesc = tc::make_smem_desc(sa + a_off, A_MN ? BK * 128 : 16, 1024);
+          const uint64_t bdesc = tc::make_smem_desc(sb + b_off, B_MN ? BK * 128 : 16, 1024);
+          const uint32_t accum = (i > 0 || k > 0) ? 1u : 0u;
+          if constexpr (sizeof(T) == 4) tc::wgmma_tf32(acc, adesc, bdesc, accum);
+          else                          tc::wgmma_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, accum);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();             // the MMAs of k-block i - 1 have retired: hand their slot back to the producer
+        tc::fence_acc(acc);
+        if (i > 0) { __syncwarp(); if (lane == 0) tc::mbar_arrive(&empty_bar[prev]); }
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      tc::wgmma_wait<0>();
+      tc::fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+
+      // ---- epilogue: this warp's 16-row band of the tile ----
+      const int r0 = m0 + wg * 64 + (warp & 3) * 16;
       const bool add_bias = bias != nullptr && sz == 0;
-      float* crow = Cbase + (int64_t)bz * c_bstride + (int64_t)m * ldc;
-      const uint32_t acc_addr = tmem_base + (uint32_t)as * kAccCols + ((uint32_t)(q * 32) << 16);
-      float* cwarp = Cbase + (int64_t)bz * c_bstride + (int64_t)(m0 + q * 32) * ldc;   // first row of this warp's 32-row band
+      if (splits > 1) {
+        // split-K: the partial tile goes to its own slice of the workspace; the last split of the tile to arrive adds the slices
+        // to C in split order (the same bits every run, whatever order the CTAs run in)
+        __shared__ unsigned int s_last;
+        float* part = ws + (int64_t)(bz * splits + sz) * M * N;
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) {
+          const int m = m0 + wg * 64 + tc::frag_row(t128, i), n = n0 + tc::frag_col(t128, i);
+          if (m < M && n < N) part[(int64_t)m * N + n] = alpha * acc[i] + (add_bias ? bias[n] : 0.f);
+        }
+        __threadfence();
+        asm volatile("bar.sync 1, %0;" ::"n"(tc::kConsumers) : "memory");
+        const int tile = (m0 / BM) + tiles_m * ((n0 / BN) + tiles_n * bz);
+        if (threadIdx.x == 0) s_last = atomicAdd(ws_cnt + tile, 1u) == (unsigned int)(splits - 1);
+        asm volatile("bar.sync 1, %0;" ::"n"(tc::kConsumers) : "memory");
+        if (s_last) {
+          __threadfence();
+          if (threadIdx.x == 0) ws_cnt[tile] = 0u;   // the stream's scratch counters are zero on entry
+          for (int e = threadIdx.x; e < BM * BN; e += tc::kConsumers) {
+            const int m = m0 + e / BN, n = n0 + e % BN;
+            if (m < M && n < N) {
+              float s = 0.f;
+              for (int z = 0; z < splits; ++z) s += __ldcg(ws + ((int64_t)(bz * splits + z) * M + m) * N + n);
+              Cbase[(int64_t)bz * c_bstride + (int64_t)m * ldc + n] += s;
+            }
+          }
+        }
+        continue;
+      }
+      float* cwarp = Cbase + (int64_t)bz * c_bstride + (int64_t)r0 * ldc;
       const bool fast = (atomic_out || beta == 0.f) && (ldc & 3) == 0 &&
                         (C16 ? (reinterpret_cast<uintptr_t>(C16) & 7) == 0 : (reinterpret_cast<uintptr_t>(cwarp + n0) & 15) == 0);
       if (fast) {
         // coalesced path: 32-column chunks through this warp's padded smem staging buffer
-        float* stage = stage_out + q * (32 * 36);
-        const int rows_valid = M - (m0 + q * 32);
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
+        float* stage = stage_out + warp * kStageFloats;
+        const int rows_valid = M - r0;
+#pragma unroll
+        for (int c = 0; c < (BN + 31) / 32; ++c) {
+          const int c0 = c * 32;
           const int cols_valid = min(N - (n0 + c0), BN - c0);
           if (cols_valid <= 0) break;   // warp-uniform
-          const int64_t off0 = (int64_t)bz * c_bstride + (int64_t)(m0 + q * 32) * ldc + n0 + c0;
-          tc::epilogue_chunk32(acc_addr + (uint32_t)c0, stage,
-                               [=](int row) -> int64_t { return row < rows_valid ? off0 + (int64_t)row * ldc : (int64_t)-1; }, cols_valid,
-                               add_bias ? bias + n0 + c0 : nullptr, alpha, relu, lane, Cbase, C16, stats ? s_stat + n0 + c0 : nullptr,
-                               stats ? s_stat + N + n0 + c0 : nullptr, atomic_out);
+          const int64_t off0 = (int64_t)bz * c_bstride + (int64_t)r0 * ldc + n0 + c0;
+          tc::frag_to_stage(stage, acc, c, lane);
+          tc::stage_to_global(stage, [=](int row) -> int64_t { return row < rows_valid ? off0 + (int64_t)row * ldc : (int64_t)-1; },
+                              cols_valid, add_bias ? bias + n0 + c0 : nullptr, alpha, relu, lane, Cbase, C16,
+                              stats ? wstat + (warp * 2) * tc::kStatW + c0 : nullptr,
+                              stats ? wstat + (warp * 2 + 1) * tc::kStatW + c0 : nullptr, atomic_out);
         }
+        if (stats) tc::stat_fold(s_stat, wstat, N, n0, min(BN, N - n0), (int)threadIdx.x);
       } else {
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        float v[16];
-        tc::tmem_ld16(acc_addr + (uint32_t)c0, v);
-        if (m < M) {
-          const int n = n0 + c0;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (n + j < N) {
-              float o = alpha * v[j] + (add_bias ? bias[n + j] : 0.f);
-              if (atomic_out) {
-                atomicAdd(crow + n + j, o);
-              } else {
-                if (beta != 0.f) o += beta * crow[n + j];
-                if (relu) o = fmaxf(o, 0.f);
-                crow[n + j] = o;
-              }
+        for (int i = 0; i < BN / 2; ++i) {
+          const int m = m0 + wg * 64 + tc::frag_row(t128, i), n = n0 + tc::frag_col(t128, i);
+          if (m < M && n < N) {
+            float* cp = Cbase + (int64_t)bz * c_bstride + (int64_t)m * ldc + n;
+            float o = alpha * acc[i] + (add_bias ? bias[n] : 0.f);
+            if (atomic_out) {
+              atomicAdd(cp, o);
+            } else {
+              if (beta != 0.f) o += beta * *cp;
+              if (relu) o = fmaxf(o, 0.f);
+              *cp = o;
             }
           }
         }
       }
-      }
-      // this warp is done reading the accumulator buffer: hand it back to the MMA warp (4 arrivals = 4 epilogue warps)
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tmem_empty_bar[as]);
     }
-    if (stats) tc::stat_flush(s_stat, stats, N, (int)threadIdx.x - 64);
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, kTmemCols);
+    if (stats) tc::stat_flush(s_stat, stats, N, (int)threadIdx.x, ws, ws_cnt);
   }
 }
 
@@ -259,8 +267,8 @@ bool make_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols,
   return r == CUDA_SUCCESS;
 }
 
-template <typename T, bool A_MN, bool B_MN>
-int launch_tc(int BN, int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
+template <typename T, bool A_MN, bool B_MN, int BN>
+int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
               int relu, float alpha, float beta, int splits, cudaStream_t stream, int nbatch = 1, int a_step = 0, int b_step = 0,
               int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr) {
   using E = Elem<T>;
@@ -271,9 +279,9 @@ int launch_tc(int BN, int M, int N, int K, const T* A, int64_t lda, const T* B, 
   if (stats) {   // the statistics come out of the coalesced epilogue path only: make sure the kernel takes it
     TFB_REQUIRE(splits <= 1 && beta == 0.f && nbatch == 1 && (ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0 && !relu && N <= 4096);
   }
-  TFB_REQUIRE(BN >= 16 && BN <= 256 && BN % 16 == 0 && (!B_MN || BN % E::kPerRow == 0));
   const int stage_bytes = kABytes + BN * 128;
-  const int stat_bytes = stats ? 2 * N * (int)sizeof(float) : 0;       // per-column accumulators behind the epilogue staging
+  // per-column accumulators and the consumer warps' per-tile statistics behind the epilogue staging
+  const int stat_bytes = stats ? (2 * N + 8 * 2 * tc::kStatW) * (int)sizeof(float) : 0;
   int stages = (kSmemMax - kSmemFixed - stat_bytes) / stage_bytes;
   if (stages > 8) stages = 8;
   const int smem_total = stages * stage_bytes + kSmemFixed + stat_bytes;
@@ -307,7 +315,7 @@ int launch_tc(int BN, int M, int N, int K, const T* A, int64_t lda, const T* B, 
       }
     } else if (beta != 1.f) { tfb_set_last_error("split-K needs beta in {0,1}"); return TFB_ERR_ARG; }
   }
-  auto kern = gemm_tc_kernel<T, A_MN, B_MN>;
+  auto kern = gemm_tc_kernel<T, A_MN, B_MN, BN>;
   static bool attr_done = false;
   if (!attr_done) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) != cudaSuccess) {
@@ -321,10 +329,36 @@ int launch_tc(int BN, int M, int N, int K, const T* A, int64_t lda, const T* B, 
   if (total > 0x7fffffff) { tfb_set_last_error("too many tiles"); return TFB_ERR_ARG; }
   int grid = (int)(total < tfb_num_sms() ? total : tfb_num_sms());
   if (g_max_ctas > 0 && grid > g_max_ctas) grid = g_max_ctas;
-  kern<<<grid, 192, smem_total, stream>>>(ma, mb, C, ldc, M, N, num_kb, kb_per_split, bias, alpha, beta, relu, atomic_out, splits, a_step,
-                                          b_step, c_bstride, tiles_m, tiles_n, (int)total, BN, stages, stats, C16);
+  // workspace of the ordered cross-CTA reductions: split-K partial tiles + one counter per output tile, or the CTAs' statistics
+  TfbScratch ws;
+  if (splits > 1) {
+    const int rc = tfb_scratch(ws, (size_t)nbatch * splits * M * N, (size_t)tiles_m * tiles_n * nbatch, stream);
+    if (rc != TFB_OK) return rc;
+  } else if (stats) {
+    const int rc = tfb_scratch(ws, (size_t)grid * 2 * N, 1, stream);
+    if (rc != TFB_OK) return rc;
+  }
+  kern<<<grid, kThreads, smem_total, stream>>>(ma, mb, C, ldc, M, N, num_kb, kb_per_split, bias, alpha, beta, relu, atomic_out, splits,
+                                               a_step, b_step, c_bstride, tiles_m, tiles_n, (int)total, stages, stats, C16, ws.f, ws.cnt);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
+}
+
+// Tile widths: multiples of 32 (K-major B), multiples of 64 (MN-major B: whole 128-byte swizzle rows); TF32 only as K-major x K-major.
+template <typename T, bool A_MN, bool B_MN>
+int launch_tc(int BN, int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
+              int relu, float alpha, float beta, int splits, cudaStream_t stream, int nbatch = 1, int a_step = 0, int b_step = 0,
+              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr) {
+#define TFB_BN(bn_) case bn_: return launch_bn<T, A_MN, B_MN, bn_>(M, N, K, A, lda, B, ldb, C, ldc, bias, relu, alpha, beta, splits, stream, \
+                                                                  nbatch, a_step, b_step, c_bstride, stats, C16)
+  if constexpr (B_MN) {
+    switch (BN) { TFB_BN(64); TFB_BN(128); TFB_BN(192); }
+  } else {
+    switch (BN) { TFB_BN(32); TFB_BN(64); TFB_BN(96); TFB_BN(128); TFB_BN(160); TFB_BN(192); }
+  }
+#undef TFB_BN
+  tfb_set_last_error("gemm_tc: unsupported tile width");
+  return TFB_ERR_ARG;
 }
 
 template <typename T>
@@ -346,7 +380,7 @@ int dispatch_major(int BN, int transA, int transB, int M, int N, int K, const T*
 // The kernel is bound by the bytes each CTA pulls from L2 per k-block ((128 + BN) * 128 B against ~42 B/clk per SM), so one CTA
 // costs ~ kb_per_split * (128 + BN) plus a fixed prologue / epilogue share (kFixed, in the same unit: ~6 k-blocks of a 128 x 128
 // tile) plus, for split-K, the fp32 atomics of its 128 x BN partial tile; the persistent grid runs ceil(CTAs / SMs) waves.
-// step = 16 (K-major B) or 64 (MN-major B: whole 128-byte swizzle rows). auto_split: the number of splits that fills one wave of
+// step = 32 (K-major B) or 64 (MN-major B: whole 128-byte swizzle rows). auto_split: the number of splits that fills one wave of
 // SMs while leaving >= 4 k-blocks per CTA (weight gradients: long contraction, few output tiles).
 int pick_bn(int M, int N, int zs, int step, int num_kb = 0, bool auto_split = false, int* splits_out = nullptr) {
   static int force_bn = -1, model_c = -2;
@@ -358,10 +392,9 @@ int pick_bn(int M, int N, int zs, int step, int num_kb = 0, bool auto_split = fa
   const int sms = (g_max_ctas > 0 && g_max_ctas < tfb_num_sms()) ? g_max_ctas : tfb_num_sms();
   int best_bn = 0, best_s = 1;
   int64_t best = -1;
-  for (int bn = step < 32 ? 32 : step; bn <= 256; bn += step) {
+  for (int bn = step; bn <= kMaxBN; bn += step) {
     int use = bn < nmax ? bn : nmax;                               // never wider than the problem
-    if (force_bn > 0) { use = ((force_bn + step - 1) / step) * step; if (use > 256) use = 256; if (use > nmax) use = nmax > 256 ? 256 : nmax; }
-    if (use > 256) continue;
+    if (force_bn > 0) { use = ((force_bn + step - 1) / step) * step; if (use > kMaxBN) use = kMaxBN; if (use > nmax) use = nmax; }
     const int64_t tiles = mt * ((N + use - 1) / use) * zs;
     int64_t cost;
     int s = 1;
@@ -391,7 +424,7 @@ int gemm_tc_any(int transA, int transB, int M, int N, int K, const T* A, int64_t
   // TMA: 16-byte aligned bases and leading dimensions.
   TFB_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0);
   TFB_REQUIRE((lda * sizeof(T)) % 16 == 0 && (ldb * sizeof(T)) % 16 == 0);
-  const int step = transB == 0 ? Elem<T>::kPerRow : 16;
+  const int step = transB == 0 ? 64 : 32;
   const int num_kb = (K + Elem<T>::kPerRow - 1) / Elem<T>::kPerRow;
   if (splits <= 0 && !stats && !C16 && !relu && (beta == 0.f || beta == 1.f)) {      // auto split-K (weight gradients)
     const int bn = pick_bn(M, N, 1, step, num_kb, true, &splits);
@@ -422,15 +455,15 @@ TFB_API int tfb_gemm_bf16_tc_wgrad_batched(int M, int N, int K, const void* A, i
   return launch_tc<T, true, true>(pick_bn(M, N, zs, 64), M, N, K, (const T*)A, lda, (const T*)B, ldb, C, ldc, nullptr, 0, 1.f, 0.f, splits, stream, nbatch, a_step, b_step, c_bstride);
 }
 
-// TF32 operands straight from fp32 storage (kind::tf32). Only the K-major x K-major case (y = x W^T) is wired up: MN-major
-// TF32 operands need the 32-byte-atom swizzle. transA must be 0 and transB 1.
+// TF32 operands straight from fp32 storage (wgmma .tf32). Only the K-major x K-major case (y = x W^T) exists: wgmma reads
+// TF32 operands K-major only. transA must be 0 and transB 1.
 TFB_API int tfb_gemm_tf32_tc(int transA, int transB, int M, int N, int K, const float* A, int64_t lda, const float* B,
                              int64_t ldb, float* C, int64_t ldc, const float* bias, int relu, float alpha, float beta,
                              int splits, cudaStream_t stream) {
   TFB_REQUIRE(M > 0 && N > 0 && K > 0 && A && B && C);
   if (transA || !transB) { tfb_set_last_error("tfb_gemm_tf32_tc: only transA=0, transB=1 is supported"); return TFB_ERR_UNSUPPORTED; }
   TFB_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0 && lda % 4 == 0 && ldb % 4 == 0);
-  return launch_tc<float, false, false>(pick_bn(M, N, 1, 16), M, N, K, A, lda, B, ldb, C, ldc, bias, relu, alpha, beta, splits, stream);
+  return launch_tc<float, false, false>(pick_bn(M, N, 1, 32), M, N, K, A, lda, B, ldb, C, ldc, bias, relu, alpha, beta, splits, stream);
 }
 
 TFB_API int tfb_gemm_bf16_tc(int transA, int transB, int M, int N, int K, const void* A, int64_t lda, const void* B,
@@ -461,9 +494,9 @@ TFB_API int tfb_gemm_bf16_tc_out16(int transB, int M, int N, int K, const void* 
                                     alpha, 0.f, 1, stream, nullptr, (__nv_bfloat16*)C16);
 }
 
-// Caps the persistent grid of the following tcgen05 GEMM launches at max_ctas CTAs (0 = no cap: one per SM). The weight-gradient
-// GEMMs run on a side stream next to the critical dx chain; with a full-chip grid they take every SM away from it (measured: the
-// step got 1.3 ms SLOWER when their split-K filled all 148 SMs), with a capped grid they use the SMs the chain leaves idle.
+// Caps the persistent grid of the following tensor-core GEMM launches at max_ctas CTAs (0 = no cap: one per SM). The weight-gradient
+// GEMMs run on a side stream next to the critical dx chain; with a full-chip grid their split-K takes every SM away from it, with a
+// capped grid they use the SMs the chain leaves idle.
 // Host-side state (not a stream operation); read at launch time, so a captured CUDA graph keeps the grid it was captured with.
 TFB_API int tfb_gemm_set_max_ctas(int max_ctas) {
   g_max_ctas = max_ctas > 0 ? max_ctas : 0;

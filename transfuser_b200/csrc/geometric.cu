@@ -93,19 +93,23 @@ __global__ void __launch_bounds__(256) gather_sum_fwd_kernel(const float* __rest
   }
 }
 
-// demb[b, cell(b,m,j), :] += dout[b,m,:]   (demb zeroed by the entry point; float atomics, duplicates are the common case)
+// demb[b, cell(b,m,j), :] += dout[b,m,:]   (demb zeroed by the entry point). Duplicate cells are the common case: one thread per
+// (b, c) owns column c of sample b's demb and adds the correspondences in (m, j) order, so the sums are the same bits every run
+// (consecutive threads = consecutive channels: the dout reads and demb updates stay coalesced).
 __global__ void __launch_bounds__(256) gather_sum_bwd_kernel(const float* __restrict__ dout, const int64_t* __restrict__ pts, float* __restrict__ demb,
                                                              int B, int h, int w, int C, int M, int P) {
-  const int64_t total = (int64_t)B * M * C;
+  const int64_t total = (int64_t)B * C;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C);
-    const int64_t bm = i / C;
-    const int b = (int)(bm / M);
-    const float g = dout[i];
-    for (int j = 0; j < P; ++j) {
-      int cell;
-      if (!resolve_cell(pts + (bm * P + j) * 2, h, w, &cell)) continue;
-      atomicAdd(demb + ((int64_t)b * h * w + cell) * C + c, g);
+    const int c = (int)(i % C), b = (int)(i / C);
+    float* col = demb + (int64_t)b * h * w * C + c;
+    for (int m = 0; m < M; ++m) {
+      const int64_t bm = (int64_t)b * M + m;
+      const float g = dout[bm * C + c];
+      for (int j = 0; j < P; ++j) {
+        int cell;
+        if (!resolve_cell(pts + (bm * P + j) * 2, h, w, &cell)) continue;
+        col[(int64_t)cell * C] += g;
+      }
     }
   }
 }
@@ -145,7 +149,7 @@ TFB_API int tfb_gather_sum_fwd(const float* emb, const int64_t* pts, float* out,
 TFB_API int tfb_gather_sum_bwd(const float* dout, const int64_t* pts, float* demb, int B, int h, int w, int C, int M, int P, cudaStream_t stream) {
   TFB_REQUIRE(dout && pts && demb && B > 0 && h > 0 && w > 0 && C > 0 && M > 0 && P > 0);
   if (cudaMemsetAsync(demb, 0, (size_t)B * h * w * C * sizeof(float), stream) != cudaSuccess) return TFB_ERR_DRIVER;
-  gather_sum_bwd_kernel<<<tfb_grid((int64_t)B * M * C, 256), 256, 0, stream>>>(dout, pts, demb, B, h, w, C, M, P);
+  gather_sum_bwd_kernel<<<tfb_grid((int64_t)B * C, 256), 256, 0, stream>>>(dout, pts, demb, B, h, w, C, M, P);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }

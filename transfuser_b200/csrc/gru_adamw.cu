@@ -61,13 +61,20 @@ gru_fwd_kernel(const float* __restrict__ z0, const float* __restrict__ target_po
   }
 }
 
-// Parameter gradients are accumulated with atomics (buffers zeroed by the launcher).
+// Parameter gradients: block b accumulates its sample's share in its own slice of `part` (every element owned by one thread),
+// and the last block adds the slices in sample order into the outputs (the same bits every run).
+constexpr int O_WHH = G3 * XIN, O_BIH = O_WHH + G3 * HID, O_BHH = O_BIH + G3, O_WOUT = O_BHH + G3, O_BOUT = O_WOUT + 3 * HID,
+              P_GRU = O_BOUT + 3;
 __global__ void __launch_bounds__(G3)
 gru_bwd_kernel(const float* __restrict__ d_wp, const float* __restrict__ save, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
-               const float* __restrict__ w_out, int steps, float* __restrict__ dz0, float* __restrict__ dw_ih, float* __restrict__ dw_hh,
-               float* __restrict__ db_ih, float* __restrict__ db_hh, float* __restrict__ dw_out, float* __restrict__ db_out) {
+               const float* __restrict__ w_out, int steps, float* __restrict__ dz0, float* __restrict__ dw_ih_out, float* __restrict__ dw_hh_out,
+               float* __restrict__ db_ih_out, float* __restrict__ db_hh_out, float* __restrict__ dw_out_out, float* __restrict__ db_out_out,
+               float* __restrict__ part, unsigned int* __restrict__ cnt) {
   __shared__ float dh[HID], dgi[G3], dgh[G3], hnew[HID], dxacc[2], dxin[XIN];
   const int b = blockIdx.x, k = threadIdx.x;
+  float* pb = part + (int64_t)b * P_GRU;
+  for (int i = k; i < P_GRU; i += blockDim.x) pb[i] = 0.f;
+  float *dw_ih = pb, *dw_hh = pb + O_WHH, *db_ih = pb + O_BIH, *db_hh = pb + O_BHH, *dw_out = pb + O_WOUT, *db_out = pb + O_BOUT;
   if (k < HID) dh[k] = 0.f;
   if (k < 2) dxacc[k] = 0.f;
   __syncthreads();
@@ -79,10 +86,10 @@ gru_bwd_kernel(const float* __restrict__ d_wp, const float* __restrict__ save, c
     // output Linear: only rows 0,1 of dxo are used
     if (k < HID) {
       dh[k] += w_out[k] * dxacc[0] + w_out[HID + k] * dxacc[1];
-      atomicAdd(&dw_out[k], dxacc[0] * hnew[k]);
-      atomicAdd(&dw_out[HID + k], dxacc[1] * hnew[k]);
+      dw_out[k] += dxacc[0] * hnew[k];
+      dw_out[HID + k] += dxacc[1] * hnew[k];
     }
-    if (k < 2) atomicAdd(&db_out[k], dxacc[k]);
+    if (k < 2) db_out[k] += dxacc[k];
     __syncthreads();
     if (k < HID) {
       const float r = sv[k], z = sv[HID + k], n = sv[2 * HID + k], hn = sv[3 * HID + k], hp = sv[4 * HID + k];
@@ -99,10 +106,10 @@ gru_bwd_kernel(const float* __restrict__ d_wp, const float* __restrict__ save, c
     {
       const float gi_k = dgi[k], gh_k = dgh[k];
 #pragma unroll
-      for (int j = 0; j < XIN; ++j) atomicAdd(&dw_ih[k * XIN + j], gi_k * sv[5 * HID + j]);
-      atomicAdd(&db_ih[k], gi_k);
-      atomicAdd(&db_hh[k], gh_k);
-      for (int j = 0; j < HID; ++j) atomicAdd(&dw_hh[k * HID + j], gh_k * sv[4 * HID + j]);
+      for (int j = 0; j < XIN; ++j) dw_ih[k * XIN + j] += gi_k * sv[5 * HID + j];
+      db_ih[k] += gi_k;
+      db_hh[k] += gh_k;
+      for (int j = 0; j < HID; ++j) dw_hh[k * HID + j] += gh_k * sv[4 * HID + j];
     }
     // input gradients
     if (k < XIN) {
@@ -120,6 +127,24 @@ gru_bwd_kernel(const float* __restrict__ d_wp, const float* __restrict__ save, c
     __syncthreads();
   }
   if (k < HID) dz0[(int64_t)b * HID + k] = dh[k];
+  __shared__ bool last;
+  __threadfence();
+  __syncthreads();
+  if (k == 0) last = atomicAdd(cnt, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  for (int i = k; i < P_GRU; i += blockDim.x) {
+    float s = 0.f;
+    for (int q = 0; q < (int)gridDim.x; ++q) s += __ldcg(part + (int64_t)q * P_GRU + i);
+    if (i < O_WHH) dw_ih_out[i] = s;
+    else if (i < O_BIH) dw_hh_out[i - O_WHH] = s;
+    else if (i < O_BHH) db_ih_out[i - O_BIH] = s;
+    else if (i < O_WOUT) db_hh_out[i - O_BHH] = s;
+    else if (i < O_BOUT) dw_out_out[i - O_WOUT] = s;
+    else db_out_out[i - O_BOUT] = s;
+  }
+  if (k == 0) *cnt = 0u;                // the stream's scratch counters are zero on entry
 }
 
 // torch.optim.AdamW semantics, scalar preparation included: torch derives 1-beta, 1-lr*wd, lr/bias_correction1 and
@@ -190,13 +215,10 @@ TFB_API int tfb_gru_bwd(const float* d_wp, const float* save, const float* w_ih,
                         float* dz0, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh, float* dw_out, float* db_out,
                         cudaStream_t stream) {
   TFB_REQUIRE(d_wp && save && w_ih && w_hh && w_out && dz0 && dw_ih && dw_hh && db_ih && db_hh && dw_out && db_out && B > 0 && steps > 0);
-  cudaMemsetAsync(dw_ih, 0, G3 * XIN * sizeof(float), stream);
-  cudaMemsetAsync(dw_hh, 0, G3 * HID * sizeof(float), stream);
-  cudaMemsetAsync(db_ih, 0, G3 * sizeof(float), stream);
-  cudaMemsetAsync(db_hh, 0, G3 * sizeof(float), stream);
-  cudaMemsetAsync(dw_out, 0, 3 * HID * sizeof(float), stream);
-  cudaMemsetAsync(db_out, 0, 3 * sizeof(float), stream);
-  gru_bwd_kernel<<<B, G3, 0, stream>>>(d_wp, save, w_ih, w_hh, w_out, steps, dz0, dw_ih, dw_hh, db_ih, db_hh, dw_out, db_out);
+  TfbScratch w;
+  const int rc = tfb_scratch(w, (size_t)B * P_GRU, 1, stream);
+  if (rc != TFB_OK) return rc;
+  gru_bwd_kernel<<<B, G3, 0, stream>>>(d_wp, save, w_ih, w_hh, w_out, steps, dz0, dw_ih, dw_hh, db_ih, db_hh, dw_out, db_out, w.f, w.cnt);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }

@@ -12,16 +12,33 @@ namespace {
 
 constexpr int kMaxC = 16;
 
-__device__ __forceinline__ void block_atomic_add(double* dst, float v, float* red) {
+// Loss sums that give the same bits every run: block b stores its sum of term k in part[b * nacc + k] (block_partial); the last
+// block (blocks_finish, called by every thread) adds the blocks' sums in block order, in fp64, to acc[k] (zeroed by the caller).
+__device__ __forceinline__ void block_partial(float* part, int nacc, int k, float v, float* red) {
   const float s = block_sum(v, red);
-  if (threadIdx.x == 0 && s != 0.f) atomicAdd(dst, (double)s);
+  if (threadIdx.x == 0) part[(int64_t)blockIdx.x * nacc + k] = s;
+}
+__device__ __forceinline__ void blocks_finish(const float* part, int nacc, double* acc, unsigned int* cnt) {
+  __shared__ bool last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(cnt, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  for (int k = threadIdx.x; k < nacc; k += blockDim.x) {
+    double s = 0.0;
+    for (unsigned int b = 0; b < gridDim.x; ++b) s += (double)__ldcg(part + (int64_t)b * nacc + k);
+    acc[k] += s;
+  }
+  if (threadIdx.x == 0) *cnt = 0u;      // the stream's scratch counters are zero on entry
 }
 
 // ---------------- cross entropy ----------------
 // acc[0] += sum_m w_m * nll_m, acc[1] += sum_m w_m, w_m = class_w[t_m] * pos_w[m % HW]
 __global__ void __launch_bounds__(256) ce_fwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ target, int64_t M, int C,
                                                      const float* __restrict__ class_w, const float* __restrict__ pos_w, int HW,
-                                                     double* __restrict__ acc) {
+                                                     double* __restrict__ acc, float* __restrict__ part, unsigned int* __restrict__ cnt) {
   __shared__ float red[32];
   float ls = 0.f, ws = 0.f;
   for (int64_t m = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; m < M; m += (int64_t)gridDim.x * blockDim.x) {
@@ -42,8 +59,9 @@ __global__ void __launch_bounds__(256) ce_fwd_kernel(const float* __restrict__ l
     ls = fmaf(w, (logf(se) + mx - lt), ls);
     ws += w;
   }
-  block_atomic_add(&acc[0], ls, red);
-  block_atomic_add(&acc[1], ws, red);
+  block_partial(part, 2, 0, ls, red);
+  block_partial(part, 2, 1, ws, red);
+  blocks_finish(part, 2, acc, cnt);
 }
 
 // dlogits = coef * w_m * (softmax - onehot), coef = (*gout) * k / (den ? max(*den, den_min) : 1)
@@ -74,7 +92,7 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const float* __restrict__ l
 
 // ---------------- L1 (optionally on sigmoid(x)) ----------------
 __global__ void __launch_bounds__(256) l1_fwd_kernel(const float* __restrict__ x, const float* __restrict__ t, int64_t n, int sigmoid,
-                                                     double* __restrict__ acc) {
+                                                     double* __restrict__ acc, float* __restrict__ part, unsigned int* __restrict__ cnt) {
   __shared__ float red[32];
   float s = 0.f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -82,7 +100,8 @@ __global__ void __launch_bounds__(256) l1_fwd_kernel(const float* __restrict__ x
     if (sigmoid) v = 1.f / (1.f + expf(-v));
     s += fabsf(v - t[i]);
   }
-  block_atomic_add(&acc[0], s, red);
+  block_partial(part, 1, 0, s, red);
+  blocks_finish(part, 1, acc, cnt);
 }
 __global__ void __launch_bounds__(256) l1_bwd_kernel(const float* __restrict__ x, const float* __restrict__ t, int64_t n, int sigmoid,
                                                      const float* __restrict__ gout, float k, float* __restrict__ dx) {
@@ -189,7 +208,8 @@ __global__ void __launch_bounds__(256) centernet_targets_kernel(const float* __r
 template <int MODE>
 __global__ void __launch_bounds__(256) centernet_loss_kernel(const float* __restrict__ pred, const float* __restrict__ tgt, int B, int HW,
                                                              const int* __restrict__ count, double* __restrict__ acc,
-                                                             const float* __restrict__ gout, float* __restrict__ dpred) {
+                                                             const float* __restrict__ gout, float* __restrict__ dpred,
+                                                             float* __restrict__ part = nullptr, unsigned int* __restrict__ cnt = nullptr) {
   __shared__ float red[32];
   constexpr int NP = 21;
   const int64_t M = (int64_t)B * HW;
@@ -277,7 +297,8 @@ __global__ void __launch_bounds__(256) centernet_loss_kernel(const float* __rest
   }
   if (MODE == 0) {
 #pragma unroll
-    for (int k = 0; k < 7; ++k) block_atomic_add(&acc[k], s[k], red);
+    for (int k = 0; k < 7; ++k) block_partial(part, 7, k, s[k], red);
+    blocks_finish(part, 7, acc, cnt);
   }
 }
 
@@ -304,7 +325,11 @@ TFB_API int tfb_ce_fwd(const float* logits, const int64_t* target, int64_t M, in
                        double* acc2, cudaStream_t stream) {
   TFB_REQUIRE(logits && target && acc2 && M > 0 && C > 0 && C <= kMaxC && HW > 0);
   if (cudaMemsetAsync(acc2, 0, 2 * sizeof(double), stream) != cudaSuccess) return TFB_ERR_DRIVER;
-  ce_fwd_kernel<<<tfb_grid(M, 256, 4), 256, 0, stream>>>(logits, target, M, C, class_w, pos_w, HW, acc2);
+  const int grid = tfb_grid(M, 256, 4);
+  TfbScratch w;
+  const int rc = tfb_scratch(w, (size_t)grid * 2, 1, stream);
+  if (rc != TFB_OK) return rc;
+  ce_fwd_kernel<<<grid, 256, 0, stream>>>(logits, target, M, C, class_w, pos_w, HW, acc2, w.f, w.cnt);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
@@ -318,7 +343,11 @@ TFB_API int tfb_ce_bwd(const float* logits, const int64_t* target, int64_t M, in
 TFB_API int tfb_l1_fwd(const float* x, const float* t, int64_t n, int sigmoid, double* acc1, cudaStream_t stream) {
   TFB_REQUIRE(x && t && acc1 && n > 0);
   if (cudaMemsetAsync(acc1, 0, sizeof(double), stream) != cudaSuccess) return TFB_ERR_DRIVER;
-  l1_fwd_kernel<<<tfb_grid(n, 256, 4), 256, 0, stream>>>(x, t, n, sigmoid, acc1);
+  const int grid = tfb_grid(n, 256, 4);
+  TfbScratch w;
+  const int rc = tfb_scratch(w, (size_t)grid, 1, stream);
+  if (rc != TFB_OK) return rc;
+  l1_fwd_kernel<<<grid, 256, 0, stream>>>(x, t, n, sigmoid, acc1, w.f, w.cnt);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
@@ -347,7 +376,11 @@ TFB_API int tfb_centernet_loss_fwd(const float* pred, const float* tgt, int B, i
                                    cudaStream_t stream) {
   TFB_REQUIRE(pred && tgt && count && acc7 && out7 && B > 0 && HW > 0);
   if (cudaMemsetAsync(acc7, 0, 7 * sizeof(double), stream) != cudaSuccess) return TFB_ERR_DRIVER;
-  centernet_loss_kernel<0><<<tfb_grid((int64_t)B * HW, 256, 2), 256, 0, stream>>>(pred, tgt, B, HW, count, acc7, nullptr, nullptr);
+  const int grid = tfb_grid((int64_t)B * HW, 256, 2);
+  TfbScratch w;
+  const int rc = tfb_scratch(w, (size_t)grid * 7, 1, stream);
+  if (rc != TFB_OK) return rc;
+  centernet_loss_kernel<0><<<grid, 256, 0, stream>>>(pred, tgt, B, HW, count, acc7, nullptr, nullptr, w.f, w.cnt);
   TFB_CHECK_LAUNCH();
   centernet_finalize_kernel<<<1, 32, 0, stream>>>(acc7, count, out7);
   TFB_CHECK_LAUNCH();

@@ -26,9 +26,11 @@ struct Finalize {
   float* running_var;
   float* zero_buf;       // optional: zero_n floats cleared by the last block (the SE pooling accumulator of the NEXT kernel on the
   int zero_n;            // stream, tfb_bn_fwd with pooling: saves the memset node)
+  double* part;          // [nsplit][nsums]: each row split's partial sums; the last block adds them in split order, so the result is
+                         // the same bits on every run (set by the launcher, see with_partials)
 };
 
-__device__ __forceinline__ void finalize_last_block(double* sums, int C, const Finalize& f) {
+__device__ __forceinline__ void finalize_last_block(double* sums, int C, const Finalize& f, int nsplit) {
   if (f.kind == 0) return;
   __shared__ bool is_last;
   __threadfence();
@@ -43,8 +45,11 @@ __device__ __forceinline__ void finalize_last_block(double* sums, int C, const F
   if (!is_last) return;
   __threadfence();
   for (int c = tid; c < C; c += nthr) {
-    const double s0 = __ldcg(sums + c);
-    const double s1 = f.nsums > C ? __ldcg(sums + C + c) : 0.0;
+    double s0 = 0.0, s1 = 0.0;
+    for (int j = 0; j < nsplit; ++j) {
+      s0 += __ldcg(f.part + (int64_t)j * f.nsums + c);
+      if (f.nsums > C) s1 += __ldcg(f.part + (int64_t)j * f.nsums + C + c);
+    }
     if (f.kind == 1) {
       const double mean = s0 / (double)f.M;
       double var = s1 / (double)f.M - mean * mean;
@@ -117,10 +122,10 @@ colreduce_kernel(const float* __restrict__ x, int64_t ldx, const float* __restri
     double t0 = 0.0, t1 = 0.0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) { t0 += sd0[j][threadIdx.x]; t1 += sd1[j][threadIdx.x]; }
-    atomicAdd(&out[c], t0);
-    if (fin.nsums > C) atomicAdd(&out[C + c], t1);
+    fin.part[(int64_t)blockIdx.y * fin.nsums + c] = t0;
+    if (fin.nsums > C) fin.part[(int64_t)blockIdx.y * fin.nsums + C + c] = t1;
   }
-  finalize_last_block(out, C, fin);
+  finalize_last_block(out, C, fin, gridDim.y);
 }
 
 // float4 variant (C % 4 == 0, 16-byte aligned rows): threadIdx.x -> one channel QUAD inside a 128-channel slab, two rows in
@@ -199,10 +204,10 @@ colreduce4_kernel(const float* __restrict__ x, int64_t ldx, const float* __restr
     double t = 0.0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) t += sd[j][tq][tv];
-    if (tv < 4) atomicAdd(&out[cc + tv], t);
-    else if (fin.nsums > C) atomicAdd(&out[C + cc + tv - 4], t);
+    if (tv < 4) fin.part[(int64_t)blockIdx.y * fin.nsums + cc + tv] = t;
+    else if (fin.nsums > C) fin.part[(int64_t)blockIdx.y * fin.nsums + C + cc + tv - 4] = t;
   }
-  finalize_last_block(out, C, fin);
+  finalize_last_block(out, C, fin, gridDim.y);
 }
 
 // Narrow matrices (C / 4 <= 128 channel quads: the 32-, 72- and 216-channel maps of the stem / stage 1 / stage 2, i.e. the LARGEST
@@ -271,10 +276,10 @@ colreduce_flat_kernel(const float* __restrict__ x, const float* __restrict__ dy,
     const int qq = i >> 3, v = i & 7;
     double sum = 0.0;
     for (int j = 0; j < RPB; ++j) sum += sd[j * C4 + qq][v];
-    if (v < 4) atomicAdd(&out[qq * 4 + v], sum);
-    else if (fin.nsums > C) atomicAdd(&out[C + qq * 4 + v - 4], sum);
+    if (v < 4) fin.part[(int64_t)blockIdx.x * fin.nsums + qq * 4 + v] = sum;
+    else if (fin.nsums > C) fin.part[(int64_t)blockIdx.x * fin.nsums + C + qq * 4 + v - 4] = sum;
   }
-  finalize_last_block(out, C, fin);
+  finalize_last_block(out, C, fin, gridDim.x);
 }
 
 // y = (x - mean) * invstd * gamma + beta (ReLU); 4 channels per thread (C % 4 == 0).
@@ -310,7 +315,7 @@ bn_apply_kernel(const float* __restrict__ x, float* __restrict__ y, int64_t tota
 __global__ void __launch_bounds__(256)
 bn_apply_pool_kernel(const float* __restrict__ x, float* __restrict__ y, int HW, int C, const float* __restrict__ mean,
                      const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
-                     float* __restrict__ pooled, float inv_hw) {
+                     float* __restrict__ pooled, float inv_hw, OrderedSum os) {
   __shared__ float4 sm[8][33];
   const int n = blockIdx.y, c = (blockIdx.x * 32 + threadIdx.x) * 4;
   float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -338,9 +343,11 @@ bn_apply_pool_kernel(const float* __restrict__ x, float* __restrict__ y, int HW,
     float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) { const float4 v = sm[j][threadIdx.x]; t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w; }
-    float* o = pooled + (int64_t)n * C + c;
-    atomicAdd(o + 0, t.x * inv_hw); atomicAdd(o + 1, t.y * inv_hw); atomicAdd(o + 2, t.z * inv_hw); atomicAdd(o + 3, t.w * inv_hw);
+    const int64_t o = (int64_t)n * C + c;
+    ordered_store(os, blockIdx.z, o + 0, t.x * inv_hw); ordered_store(os, blockIdx.z, o + 1, t.y * inv_hw);
+    ordered_store(os, blockIdx.z, o + 2, t.z * inv_hw); ordered_store(os, blockIdx.z, o + 3, t.w * inv_hw);
   }
+  ordered_finish(os, pooled);
 }
 
 // ---- BatchNorm forward when the statistics were accumulated by the PRODUCER's epilogue (tfb_gemm_bf16_tc_stats, tfb_conv3x3_tc_strided):
@@ -406,7 +413,7 @@ __global__ void __launch_bounds__(256)
 bn_apply_pool_stats_kernel(const float* __restrict__ x, float* __restrict__ y, int HW, int C, int64_t M, const double* __restrict__ stats,
                            const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum, int relu,
                            float* __restrict__ save_mean, float* __restrict__ save_invstd, float* __restrict__ running_mean,
-                           float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw) {
+                           float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw, OrderedSum os) {
   __shared__ __align__(16) float s_par[2 * kBnStatsMaxC];
   float* s_scale = s_par;
   float* s_shift = s_par + kBnStatsMaxC;
@@ -433,9 +440,11 @@ bn_apply_pool_stats_kernel(const float* __restrict__ x, float* __restrict__ y, i
     float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) { const float4 v = sm[j][threadIdx.x]; t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w; }
-    float* o = pooled + (int64_t)n * C + c;
-    atomicAdd(o + 0, t.x * inv_hw); atomicAdd(o + 1, t.y * inv_hw); atomicAdd(o + 2, t.z * inv_hw); atomicAdd(o + 3, t.w * inv_hw);
+    const int64_t o = (int64_t)n * C + c;
+    ordered_store(os, blockIdx.z, o + 0, t.x * inv_hw); ordered_store(os, blockIdx.z, o + 1, t.y * inv_hw);
+    ordered_store(os, blockIdx.z, o + 2, t.z * inv_hw); ordered_store(os, blockIdx.z, o + 3, t.w * inv_hw);
   }
+  ordered_finish(os, pooled);
 }
 
 // bn_apply_pool_stats_kernel for narrow maps (C / 4 <= 128): whole pixel rows of one sample per block iteration, every lane busy
@@ -444,7 +453,7 @@ __global__ void __launch_bounds__(256)
 bn_apply_pool_stats_flat_kernel(const float* __restrict__ x, float* __restrict__ y, int HW, int C, int64_t M, const double* __restrict__ stats,
                                 const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum, int relu,
                                 float* __restrict__ save_mean, float* __restrict__ save_invstd, float* __restrict__ running_mean,
-                                float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw) {
+                                float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw, OrderedSum os) {
   __shared__ __align__(16) float s_par[2 * 512];
   float* s_scale = s_par;
   float* s_shift = s_par + 512;
@@ -471,9 +480,11 @@ bn_apply_pool_stats_flat_kernel(const float* __restrict__ x, float* __restrict__
   if (t < C4) {
     float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int j = 0; j < RPB; ++j) { const float4 v = sm[j * C4 + t]; s4.x += v.x; s4.y += v.y; s4.z += v.z; s4.w += v.w; }
-    float* o = pooled + (int64_t)n * C + t * 4;
-    atomicAdd(o + 0, s4.x * inv_hw); atomicAdd(o + 1, s4.y * inv_hw); atomicAdd(o + 2, s4.z * inv_hw); atomicAdd(o + 3, s4.w * inv_hw);
+    const int64_t o = (int64_t)n * C + t * 4;
+    ordered_store(os, blockIdx.x, o + 0, s4.x * inv_hw); ordered_store(os, blockIdx.x, o + 1, s4.y * inv_hw);
+    ordered_store(os, blockIdx.x, o + 2, s4.z * inv_hw); ordered_store(os, blockIdx.x, o + 3, s4.w * inv_hw);
   }
+  ordered_finish(os, pooled);
 }
 
 // dx = gamma * invstd * (g - sum_g/M - xhat * sum_gx/M);  block 0 also writes dgamma = sum_gx, dbeta = sum_g.
@@ -656,10 +667,10 @@ ln_bwd_param_kernel(const float* __restrict__ x, const float* __restrict__ dy, i
     float ta = 0.f, tb = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) { ta += sg[j][threadIdx.x]; tb += sb[j][threadIdx.x]; }
-    atomicAdd(&sums[c], (double)tb);
-    atomicAdd(&sums[C + c], (double)ta);
+    fin.part[(int64_t)blockIdx.y * fin.nsums + c] = (double)tb;
+    fin.part[(int64_t)blockIdx.y * fin.nsums + C + c] = (double)ta;
   }
-  finalize_last_block(sums, C, fin);
+  finalize_last_block(sums, C, fin, gridDim.y);
 }
 
 // Backward prologue of a dense layer, one pass over dy [M, C]:  g = relu ? dy * (y > 0) : dy;  optional outputs: g in fp32, g in
@@ -687,9 +698,9 @@ grad_prep_kernel(const float* __restrict__ dy, const float* __restrict__ y, floa
       float t = 0.f;
 #pragma unroll
       for (int j = 0; j < 8; ++j) t += sm[j][threadIdx.x];
-      atomicAdd(&sums[c], (double)t);
+      fin.part[(int64_t)blockIdx.y * fin.nsums + c] = (double)t;
     }
-    finalize_last_block(sums, C, fin);
+    finalize_last_block(sums, C, fin, gridDim.y);
   }
 }
 
@@ -712,6 +723,14 @@ __global__ void __launch_bounds__(256) scale_gate_kernel(const float* __restrict
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// fin.part for a reduction with nsplit row splits, in the stream's scratch.
+int alloc_partials(Finalize& fin, int64_t nsplit, cudaStream_t stream) {
+  TfbScratch w;
+  const int rc = tfb_scratch(w, (size_t)(2 * nsplit * fin.nsums), 0, stream);   // doubles = 2 floats each
+  fin.part = reinterpret_cast<double*>(w.f);
+  return rc;
+}
+
 int colreduce_min_rows() {           // rows per thread below which a column reduction is not split further
   static int v = -1;
   if (v < 0) { const char* e = getenv("TFB_COLREDUCE_ROWS"); v = e ? atoi(e) : 16; if (v < 1) v = 1; }
@@ -733,6 +752,7 @@ int launch_colreduce(const float* x, int64_t ldx, const float* dy, int64_t M, in
   const bool vec = C % 4 == 0 && ldx % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (!dy || (reinterpret_cast<uintptr_t>(dy) & 15) == 0) &&
                    (!ymask || (reinterpret_cast<uintptr_t>(ymask) & 15) == 0);
   dim3 block(32, 8);
+  int rc;
   if (vec && C / 4 <= 128 && ldx == C && M >= 4096) {
     // narrow and tall: whole rows per block, every lane busy (see colreduce_flat_kernel)
     const int rpb = 256 / (C / 4);
@@ -740,19 +760,21 @@ int launch_colreduce(const float* x, int64_t ldx, const float* dy, int64_t M, in
     const int64_t cap = (int64_t)tfb_num_sms() * 4;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
+    if ((rc = alloc_partials(fin, blocks, stream)) != TFB_OK) return rc;
     colreduce_flat_kernel<MODE><<<(int)blocks, 256, 0, stream>>>(x, dy, M, C, out, mean, invstd, gamma, beta, relu, ymask, fin);
-    return 0;
-  }
-  if (vec) {
+  } else if (vec) {
     const int slabs = (C / 4 + 31) / 32;
     dim3 grid(slabs, colreduce_splits(M, slabs));
+    if ((rc = alloc_partials(fin, grid.y, stream)) != TFB_OK) return rc;
     colreduce4_kernel<MODE><<<grid, block, 0, stream>>>(x, ldx, dy, M, C, out, mean, invstd, gamma, beta, relu, ymask, fin);
   } else {
     const int slabs = (C + 31) / 32;
     dim3 grid(slabs, colreduce_splits(M, slabs));
+    if ((rc = alloc_partials(fin, grid.y, stream)) != TFB_OK) return rc;
     colreduce_kernel<MODE><<<grid, block, 0, stream>>>(x, ldx, dy, M, C, out, mean, invstd, gamma, beta, relu, ymask, fin);
   }
-  return 0;
+  TFB_CHECK_LAUNCH();
+  return TFB_OK;
 }
 
 }  // namespace
@@ -769,14 +791,17 @@ TFB_API int tfb_bn_fwd(const float* x, float* y, int64_t M, int C, const float* 
   TFB_REQUIRE(x && y && gamma && beta && save_mean && save_invstd && sums_ws && M > 0 && C > 0 && C % 4 == 0);
   TFB_REQUIRE(!pooled || (pool_batch > 0 && M % pool_batch == 0 && !y16_bf16 && !residual));
   Finalize fin = {1, 2 * C, M, eps, momentum, save_mean, save_invstd, running_mean, running_var, pooled, pooled ? pool_batch * C : 0};
-  launch_colreduce<0>(x, C, nullptr, M, C, sums_ws, nullptr, nullptr, nullptr, nullptr, 0, nullptr, fin, stream);
-  TFB_CHECK_LAUNCH();
+  const int rc = launch_colreduce<0>(x, C, nullptr, M, C, sums_ws, nullptr, nullptr, nullptr, nullptr, 0, nullptr, fin, stream);
+  if (rc != TFB_OK) return rc;
   if (pooled) {
     const int HW = (int)(M / pool_batch);
     int splits = (HW + 255) / 256;
     if (splits > 32) splits = 32;
     dim3 grid((C / 4 + 31) / 32, pool_batch, splits), block(32, 8);
-    bn_apply_pool_kernel<<<grid, block, 0, stream>>>(x, y, HW, C, save_mean, save_invstd, gamma, beta, relu, pooled, 1.f / (float)HW);
+    OrderedSum os;
+    const int rc2 = ordered_alloc(os, splits, (int64_t)pool_batch * C, stream);
+    if (rc2 != TFB_OK) return rc2;
+    bn_apply_pool_kernel<<<grid, block, 0, stream>>>(x, y, HW, C, save_mean, save_invstd, gamma, beta, relu, pooled, 1.f / (float)HW, os);
     TFB_CHECK_LAUNCH();
     return TFB_OK;
   }
@@ -805,14 +830,20 @@ TFB_API int tfb_bn_fwd_stats(const float* x, float* y, int64_t M, int C, const f
       const int cap = (4 * tfb_num_sms() + pool_batch - 1) / pool_batch;
       if (sp > cap) sp = cap;
       if (sp < 1) sp = 1;
+      OrderedSum os;
+      const int rc = ordered_alloc(os, sp, (int64_t)pool_batch * C, stream);
+      if (rc != TFB_OK) return rc;
       bn_apply_pool_stats_flat_kernel<<<dim3(sp, pool_batch), 256, 0, stream>>>(x, y, HW, C, M, stats, gamma, beta, eps, momentum, relu, save_mean,
-                                                                               save_invstd, running_mean, running_var, pooled, 1.f / (float)HW);
+                                                                               save_invstd, running_mean, running_var, pooled, 1.f / (float)HW, os);
       TFB_CHECK_LAUNCH();
       return TFB_OK;
     }
     dim3 grid((C / 4 + 31) / 32, pool_batch, splits), block(32, 8);
+    OrderedSum os;
+    const int rc = ordered_alloc(os, splits, (int64_t)pool_batch * C, stream);
+    if (rc != TFB_OK) return rc;
     bn_apply_pool_stats_kernel<<<grid, block, 0, stream>>>(x, y, HW, C, M, stats, gamma, beta, eps, momentum, relu, save_mean, save_invstd,
-                                                              running_mean, running_var, pooled, 1.f / (float)HW);
+                                                              running_mean, running_var, pooled, 1.f / (float)HW, os);
     TFB_CHECK_LAUNCH();
     return TFB_OK;
   }
@@ -852,24 +883,28 @@ static int bn_bwd_impl(const float* x, const float* dy, float* dx, int64_t M, in
     se_gate = se_dpool = nullptr;
   }
   if (se_gate) {
+    int rc;
     if (C / 4 <= 128 && M >= 4096) {            // as launch_colreduce picks
       const int rpb = 256 / (C / 4);
       int64_t blocks = ceil_div64(M, (int64_t)rpb * 8);
       const int64_t cap = (int64_t)tfb_num_sms() * 4;
       if (blocks > cap) blocks = cap;
       if (blocks < 1) blocks = 1;
+      if ((rc = alloc_partials(fin, blocks, stream)) != TFB_OK) return rc;
       colreduce_flat_kernel<1><<<(int)blocks, 256, 0, stream>>>(x, dy, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu, ymask, fin,
                                                                se_gate, se_dpool, hw);
     } else {
       const int slabs = (C / 4 + 31) / 32;
       dim3 grid(slabs, colreduce_splits(M, slabs)), block(32, 8);
+      if ((rc = alloc_partials(fin, grid.y, stream)) != TFB_OK) return rc;
       colreduce4_kernel<1><<<grid, block, 0, stream>>>(x, C, dy, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu, ymask, fin, se_gate,
                                                        se_dpool, hw);
     }
+    TFB_CHECK_LAUNCH();
   } else {
-    launch_colreduce<1>(x, C, dy, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu, ymask, fin, stream);
+    const int rc = launch_colreduce<1>(x, C, dy, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu, ymask, fin, stream);
+    if (rc != TFB_OK) return rc;
   }
-  TFB_CHECK_LAUNCH();
   bn_bwd_apply_kernel<<<tfb_grid(M * C / 4, 256), 256, 0, stream>>>(x, dy, dx, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu,
                                                                 dgamma, dbeta, (__nv_bfloat16*)dx16_bf16, ymask, gmasked, se_gate, se_dpool, hw);
   TFB_CHECK_LAUNCH();
@@ -910,9 +945,7 @@ TFB_API int tfb_bn_bwd_se(const float* x, const float* dy, float* dx, int64_t M,
 TFB_API int tfb_colsum(const float* x, int64_t ldx, int64_t M, int C, float* out, double* sums_ws, cudaStream_t stream) {
   TFB_REQUIRE(x && out && sums_ws && M > 0 && C > 0 && ldx >= C);
   Finalize fin = {3, C, M, 0.f, 0.f, out, nullptr, nullptr, nullptr};
-  launch_colreduce<0>(x, ldx, nullptr, M, C, sums_ws, nullptr, nullptr, nullptr, nullptr, 0, nullptr, fin, stream);
-  TFB_CHECK_LAUNCH();
-  return TFB_OK;
+  return launch_colreduce<0>(x, ldx, nullptr, M, C, sums_ws, nullptr, nullptr, nullptr, nullptr, 0, nullptr, fin, stream);
 }
 
 // See grad_prep_kernel. Any of y / g32 / g16_bf16 / dbias may be null; sums_ws (C doubles) is needed when dbias is given.
@@ -922,6 +955,10 @@ TFB_API int tfb_grad_prep(const float* dy, const float* y, float* g32, void* g16
   const int slabs = (C + 31) / 32;
   dim3 grid(slabs, colreduce_splits(M, slabs)), block(32, 8);
   Finalize fin = {dbias ? 3 : 0, C, M, 0.f, 0.f, dbias, nullptr, nullptr, nullptr};
+  if (dbias) {
+    const int rc = alloc_partials(fin, grid.y, stream);
+    if (rc != TFB_OK) return rc;
+  }
   grad_prep_kernel<<<grid, block, 0, stream>>>(dy, y, g32, (__nv_bfloat16*)g16_bf16, dbias ? sums_ws : nullptr, M, C, fin);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
@@ -948,6 +985,8 @@ TFB_API int tfb_layernorm_bwd(const float* x, const float* dy, float* dx, int64_
   if (splits < 1) splits = 1;
   dim3 grid(slabs, splits), block(32, 8);
   Finalize fin = {2, 2 * C, R, 0.f, 0.f, dbeta, dgamma, nullptr, nullptr};
+  const int rc = alloc_partials(fin, grid.y, stream);
+  if (rc != TFB_OK) return rc;
   ln_bwd_param_kernel<<<grid, block, 0, stream>>>(x, dy, R, C, save_mean, save_rstd, sums_ws, fin);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
@@ -980,6 +1019,8 @@ TFB_API int tfb_add_dropout_ln_bwd(const float* xnew, const float* dh, const flo
   if (splits < 1) splits = 1;
   dim3 grid(slabs, splits), block(32, 8);
   Finalize fin = {2, 2 * C, R, 0.f, 0.f, dbeta, dgamma, nullptr, nullptr};
+  const int rc = alloc_partials(fin, grid.y, stream);
+  if (rc != TFB_OK) return rc;
   ln_bwd_param_kernel<<<grid, block, 0, stream>>>(xnew, dh, R, C, save_mean, save_rstd, sums_ws, fin);
   TFB_CHECK_LAUNCH();
   return TFB_OK;

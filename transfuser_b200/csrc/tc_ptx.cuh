@@ -1,10 +1,13 @@
-// Inline-PTX wrappers for the Blackwell (sm_100a) async machinery: mbarrier, TMA (cp.async.bulk.tensor),
-// TMEM allocation, tcgen05.mma / commit / ld, and UMMA shared-memory / instruction descriptors.
+// Inline-PTX wrappers for the Hopper (sm_90a) async machinery: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA
+// (wgmma.mma_async with register accumulators, wgmma.cuh) and its shared-memory matrix descriptors, plus the register-fragment
+// epilogue shared by the tensor-core kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace tc {
 
@@ -52,109 +55,59 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3,
-                                            int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::
-          "r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
 
-// ---------------- TMEM / tcgen05 ----------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// tcgen05.commit: arrive on an mbarrier when all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; kind::tf32 (fp32 storage, 10-bit mantissa used) or kind::f16 (bf16/fp16).
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp gets lane (lane_base + t), columns [col, col+16).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---------------- wgmma ----------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses of the accumulator registers across wgmma_fence / wgmma_wait.
+template <int K> __device__ __forceinline__ void fence_acc(float (&d)[K]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < K; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// generic-proxy writes to shared memory (st.shared, cp.async) -> visible to wgmma / TMA (async proxy)
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// Same, without the wait: issue several loads back to back, then tmem_ld_wait() once.
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// Register fragment of a 64 x N wgmma accumulator: element i of thread t (t = thread index in its warpgroup) holds row
+// frag_row(t, i) and column frag_col(t, i); elements 2j and 2j + 1 are adjacent columns of the same row.
+__device__ __forceinline__ int frag_row(int t, int i) { return (t >> 5) * 16 + ((t & 31) >> 2) + ((i >> 1) & 1) * 8; }
+__device__ __forceinline__ int frag_col(int t, int i) { return (i >> 2) * 8 + (t & 3) * 2 + (i & 1); }
 
 // fp32 vector reduction into global memory (sm_90+): four consecutive floats, 16-byte aligned, one L2 transaction per lane instead of 4
 __device__ __forceinline__ void red_add_v4(float* p, float4 v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
-// Epilogue helper: one warp moves its 32 accumulator rows x 32 columns TMEM -> registers -> padded smem (row stride 36 floats:
-// conflict-free 16-byte accesses both ways) -> global memory with COALESCED row segments (4 rows per instruction, 128 bytes of fp32
-// or 64 bytes of bf16 per row), applying o = alpha*acc + bias (ReLU). `stage` is this warp's private 32 x 36 float buffer.
-// `row_off(row)` returns the ELEMENT offset of accumulator row `row` (0..31) in the output (a multiple of 4) or -1 for rows that
+// Epilogue, part 1: columns [32c, 32c + 32) of this warp's 16 accumulator rows (fragment -> padded smem, row stride 36 floats).
+// c must be a compile-time constant after unrolling so that the accumulator stays in registers.
+template <int K>
+__device__ __forceinline__ void frag_to_stage(float* stage, const float (&acc)[K], int c, int lane) {
+  const int r = lane >> 2, cc = (lane & 3) * 2;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = c * 4 + jj;
+    if (j * 4 < K) {
+      *reinterpret_cast<float2*>(stage + r * 36 + jj * 8 + cc) = make_float2(acc[j * 4], acc[j * 4 + 1]);
+      *reinterpret_cast<float2*>(stage + (r + 8) * 36 + jj * 8 + cc) = make_float2(acc[j * 4 + 2], acc[j * 4 + 3]);
+    }
+  }
+  __syncwarp();
+}
+
+// Epilogue, part 2: one warp writes the 16 x 32 staged block to global memory with COALESCED row segments (4 rows per
+// instruction, 128 bytes of fp32 or 64 bytes of bf16 per row), applying o = alpha*acc + bias (ReLU).
+// `row_off(row)` returns the ELEMENT offset of staged row `row` (0..15) in the output (a multiple of 4) or -1 for rows that
 // must not be written; columns >= cols_valid are not written. The result goes to out32 (fp32) or, when out16 is given, to out16
 // (bf16, round-to-nearest-even) at the same element offsets. atomic: the fp32 values are ADDED to out32 (split-K partial tiles).
-// stat_sum / stat_sq (optional, fp32 accumulators in SHARED memory, this chunk's column 0): per-column sum and sum of squares of
-// the values written (rows with offset -1 contribute nothing) — the training-mode BatchNorm statistics of a conv / GEMM output
-// come out of its epilogue instead of a separate read pass over the tensor. The CTA accumulates over all of its tiles and flushes
-// once (stat_flush) with one fp64 global atomic per column: a first version that issued global atomics per warp and chunk
-// serialised thousands of same-address atomics on the 72-channel, 70 400-row stage-1 GEMMs and cost more than the pass it removed.
+// stat_sum / stat_sq (optional, this warp's per-tile buffers in SHARED memory, this chunk's column 0): per-column sum and sum of
+// squares of the values written (rows with offset -1 contribute nothing) — the training-mode BatchNorm statistics of a conv / GEMM
+// output come out of its epilogue instead of a separate read pass over the tensor. They are STORED (each column of a tile belongs
+// to one chunk); stat_fold adds the warps' buffers into the CTA's accumulators in warp order, and stat_flush reduces the CTAs in
+// CTA order, so the statistics are the same bits on every run.
 template <class RowOff>
-__device__ __forceinline__ void epilogue_chunk32(uint32_t taddr, float* stage, RowOff row_off, int cols_valid, const float* bias,
-                                                 float alpha, int relu, int lane, float* out32, __nv_bfloat16* out16 = nullptr,
-                                                 float* stat_sum = nullptr, float* stat_sq = nullptr, int atomic = 0) {
-  uint32_t r[32];
-  tmem_ld16_nowait(taddr, r);
-  tmem_ld16_nowait(taddr + 16, r + 16);
-  tmem_ld_wait();
-  float* srow = stage + lane * 36;
-#pragma unroll
-  for (int j = 0; j < 32; j += 4)
-    *reinterpret_cast<float4*>(srow + j) = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                                       __uint_as_float(r[j + 3]));
-  __syncwarp();
+__device__ __forceinline__ void stage_to_global(const float* stage, RowOff row_off, int cols_valid, const float* bias, float alpha,
+                                                int relu, int lane, float* out32, __nv_bfloat16* out16 = nullptr,
+                                                float* stat_sum = nullptr, float* stat_sq = nullptr, int atomic = 0) {
   const int c4 = (lane & 7) * 4, rsub = lane >> 3;
   float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
   if (bias) {
@@ -165,7 +118,7 @@ __device__ __forceinline__ void epilogue_chunk32(uint32_t taddr, float* stage, R
   }
   float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
+  for (int i = 0; i < 4; ++i) {
     const int row = i * 4 + rsub;
     float4 v = *reinterpret_cast<const float4*>(stage + row * 36 + c4);
     v.x = fmaf(alpha, v.x, bv.x); v.y = fmaf(alpha, v.y, bv.y); v.z = fmaf(alpha, v.z, bv.z); v.w = fmaf(alpha, v.w, bv.w);
@@ -218,43 +171,66 @@ __device__ __forceinline__ void epilogue_chunk32(uint32_t taddr, float* stage, R
     if (lane < 8) {
 #pragma unroll
       for (int q = 0; q < 4; ++q)
-        if (c4 + q < cols_valid) { atomicAdd(stat_sum + c4 + q, s1[q]); atomicAdd(stat_sq + c4 + q, s2[q]); }
+        if (c4 + q < cols_valid) { stat_sum[c4 + q] = s1[q]; stat_sq[c4 + q] = s2[q]; }
     }
   }
   __syncwarp();
 }
 
-// The four epilogue warps (128 threads, named barrier 1) clear / flush the CTA's per-column statistics accumulators s_stat[2][n]
-// (shared) into stats[2][n] (global fp64: [sum | sum of squares]). t = thread index among the 128 epilogue threads.
+// Deterministic per-column statistics. The consumer warps (kConsumers threads, named barrier 1) own
+//   s_stat[2][n]          the CTA's accumulators (shared), cleared by stat_clear,
+//   wstat[8][2][kStatW]   one per-tile buffer per consumer warp (shared), written by stage_to_global.
+// stat_fold adds columns [0, ncols) of the eight warp buffers, in warp order, into s_stat + col0 (and s_stat + n + col0);
+// stat_flush writes the CTA's accumulators to its row of ws[gridDim.x][2n] and the last CTA to arrive (counter *cnt, zero on
+// entry, reset on exit) adds the rows in CTA order, in fp64, into stats[2][n] (global: [sum | sum of squares]).
+// t = thread index among the consumer threads.
+constexpr int kConsumers = 256;
+constexpr int kStatW = 256;                    // widest tile
 __device__ __forceinline__ void stat_clear(float* s_stat, int n, int t) {
-  for (int i = t; i < 2 * n; i += 128) s_stat[i] = 0.f;
-  asm volatile("bar.sync 1, 128;" ::: "memory");
+  for (int i = t; i < 2 * n; i += kConsumers) s_stat[i] = 0.f;
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
 }
-__device__ __forceinline__ void stat_flush(const float* s_stat, double* stats, int n, int t) {
-  asm volatile("bar.sync 1, 128;" ::: "memory");
-  for (int i = t; i < 2 * n; i += 128) {
-    const float v = s_stat[i];
-    if (v != 0.f) atomicAdd(stats + i, (double)v);
+__device__ __forceinline__ void stat_fold(float* s_stat, const float* wstat, int n, int col0, int ncols, int t) {
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+  for (int j = t; j < 2 * ncols; j += kConsumers) {
+    const int q = j / ncols, c = j - q * ncols;
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += wstat[(w * 2 + q) * kStatW + c];
+    s_stat[q * n + col0 + c] += s;
   }
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+}
+__device__ __forceinline__ void stat_flush(const float* s_stat, double* stats, int n, int t, float* ws, unsigned int* cnt) {
+  __shared__ unsigned int s_last;
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+  for (int i = t; i < 2 * n; i += kConsumers) ws[(int64_t)blockIdx.x * 2 * n + i] = s_stat[i];
+  __threadfence();
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+  if (t == 0) s_last = atomicAdd(cnt, 1u) == gridDim.x - 1;
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+  if (!s_last) return;
+  __threadfence();
+  for (int i = t; i < 2 * n; i += kConsumers) {
+    double s = 0.0;
+    for (unsigned int b = 0; b < gridDim.x; ++b) s += (double)__ldcg(ws + (int64_t)b * 2 * n + i);
+    stats[i] += s;
+  }
+  if (t == 0) *cnt = 0u;               // the stream's scratch counters are zero on entry
 }
 
 // ---------------- descriptors ----------------
-// Shared-memory matrix descriptor, SWIZZLE_128B (layout_type 2), descriptor version 1 (Blackwell).
-//   K-major operand : rows of 128 B (the K extent of one stage), 8-row groups 1024 B apart -> SBO = 1024, LBO = 16 (ignored)
+// wgmma shared-memory matrix descriptor (sm_90): start address, leading / stride byte offsets (>> 4), swizzle mode in bits 62-63
+// (1 = 128B, 2 = 64B, 3 = 32B); stage buffers are 1024-byte aligned, so the base-offset field stays 0.
+//   K-major operand : rows of 128 B (64 B for SWIZZLE_64B), 8-row groups SBO bytes apart; LBO unused (1)
 //   MN-major operand: 128 B of MN-contiguous elements per K row, 8-row K groups 1024 B apart (SBO), next 128 B MN chunk at LBO
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, int swizzle_bytes = 128) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // version
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+  d |= (uint64_t)(swizzle_bytes == 128 ? 1 : swizzle_bytes == 64 ? 2 : 3) << 62;
   return d;
-}
-
-// Instruction descriptor (upper 32 bits of idescE): fp32 accumulate, A/B format (0 f16, 1 bf16, 2 tf32), majors, N>>3, M>>4.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t fmt, uint32_t a_mn_major, uint32_t b_mn_major, uint32_t m, uint32_t n) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
 }
 
 }  // namespace tc

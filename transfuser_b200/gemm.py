@@ -5,11 +5,11 @@ import torch
 
 from . import _lib
 
-# 'simt' (exact fp32 CUDA cores: the parity mode and the import-time default), 'bf16' (tcgen05 kind::f16 tensor cores, fp32
+# 'simt' (exact fp32 CUDA cores: the parity mode and the import-time default), 'bf16' (wgmma bf16 tensor cores, fp32
 # accumulate: the throughput mode bench.py / Trainer select), 'bf16x3' / 'bf16x6' (the tensor-core PARITY modes: every fp32 operand
-# is split into 2 / 3 bf16 terms — 16 / 24 of its mantissa bits — and a product runs as 3 / 6 tcgen05 bf16 GEMMs, smallest terms
+# is split into 2 / 3 bf16 terms — 16 / 24 of its mantissa bits — and a product runs as 3 / 6 tensor-core bf16 GEMMs, smallest terms
 # first, accumulated in fp32: ~1e-5 relative per product for x3, fp32-grade for x6; the sidecar / fusion machinery of 'bf16' is
-# off), 'tf32' (tcgen05 kind::tf32 for K-major operands only)
+# off), 'tf32' (wgmma tf32 for K-major operands only)
 MODE = os.environ.get('TFB_GEMM', 'simt')
 MULTI_TERM = {'bf16x3': 2, 'bf16x6': 3}      # mode -> bf16 terms per operand
 
@@ -50,7 +50,7 @@ def gemm(a, b, out, trans_a=False, trans_b=False, bias=None, relu=False, alpha=1
 
 
 def x3_ok(M, N, K, trans_a, trans_b):
-    """Shapes the three-term bf16 product takes: the tcgen05 kernel's minimum tile and 16-byte aligned rows of the (contiguous)
+    """Shapes the three-term bf16 product takes: the tensor-core kernel's minimum tile and 16-byte aligned rows of the (contiguous)
     split operands; everything else stays on the exact fp32 kernel."""
     lda, ldb = (M if trans_a else K), (K if trans_b else N)
     return M >= 16 and N >= 16 and K >= 16 and lda % 8 == 0 and ldb % 8 == 0
@@ -68,7 +68,7 @@ def split_bf16(x, terms=None):
 
 def gemm_x3(a, b, out, trans_a=False, trans_b=False, bias=None, relu=False, alpha=1.0, beta=0.0):
     """out = alpha * op(a) @ op(b) + beta*out (+bias) (relu) from pre-split operands a = (a0, a1[, a2]), b = (b0, b1[, b2]) (largest
-    term first): the term-by-term tcgen05 bf16 GEMMs whose order i + j is below the number of terms (3 products for 2 terms, 6 for 3;
+    term first): the term-by-term tensor-core bf16 GEMMs whose order i + j is below the number of terms (3 products for 2 terms, 6 for 3;
     the dropped ones are below 2^-16 / 2^-24 of the result), smallest first, accumulated in fp32 in `out` (reduction epilogue)."""
     M, N = out.shape
     K = a[0].shape[0] if trans_a else a[0].shape[1]
@@ -132,7 +132,7 @@ def weight_bf16(w):
 
 
 def tc_ok(M, N, K, *lds):
-    """Shapes the tcgen05 bf16 kernel takes (TMA: 16-byte aligned leading dimensions); everything else runs on the SIMT kernel."""
+    """Shapes the tensor-core bf16 kernel takes (TMA: 16-byte aligned leading dimensions); everything else runs on the SIMT kernel."""
     return MODE == 'bf16' and M >= 32 and N >= 16 and K >= 16 and all(ld % 8 == 0 for ld in lds)
 
 

@@ -1,9 +1,9 @@
-"""B200-native `LidarCenterNet` training forward — drop-in for /root/reference/team_code_transfuser/model.py:538-805.
+"""H100-native `LidarCenterNet` training forward — drop-in for team_code_transfuser/model.py:538-805.
 
 Same constructor and `forward(...) -> dict of the 11 scalar losses` contract (keys = config.detailed_losses), same
 parameter names (`_model.*`, `seg_decoder.*`, `depth_decoder.*`, `pred_bev.*`, `head.*_head.*`, `join.*`, `decoder.*`,
 `output.*`), so train.py's loop (`loss.backward()`, `optimizer.step()`, `state_dict()`) runs unchanged. The nn.* members
-are parameter containers; all compute goes through transfuser_b200.ops (hand-written sm_100a kernels).
+are parameter containers; all compute goes through transfuser_b200.ops (hand-written sm_90a kernels).
 `forward_ego` (model.py:685-731: waypoints + decoded boxes for the driving agent) runs the same kernels in eval mode plus the
 one-launch CenterNet decode; the agent-side control / visualisation members (control_pid, visualize_model_io) are out of scope."""
 import numpy as np

@@ -1,5 +1,5 @@
 """torch.autograd.Function wrappers over the C-ABI kernels (include/tfb200.h): every forward AND backward below is a
-hand-written sm_100a kernel launch; torch supplies device memory, the current stream and the autograd graph only.
+hand-written sm_90a kernel launch; torch supplies device memory, the current stream and the autograd graph only.
 
 Activations are NHWC fp32 ([N, H, W, C], contiguous); parameters keep the reference's PyTorch layouts so that the
 reference's state_dicts load unchanged (SURVEY.md §8b)."""
@@ -94,12 +94,12 @@ QKV_FUSED = os.environ.get('TFB_QKV_FUSED', '1') == '1'           # one q|k|v GE
 BN_ADD_FUSED = os.environ.get('TFB_BN_ADD_FUSED', '1') == '1'     # conv3.bn + shortcut add + ReLU as one BatchNorm call
 SE_POOL_FUSED = os.environ.get('TFB_SE_POOL_FUSED', '1') == '1'   # SE average pool inside the preceding BatchNorm's pass
 SE_FUSED_BWD = os.environ.get('TFB_SE_FUSED_BWD', '1') == '1'   # tfb_se_mlp_bwd (2 launches) instead of 8 small ones
-CONV_S2_TC = os.environ.get('TFB_CONV_S2_TC', '1') == '1'       # bf16 mode: stride-2 3x3 convs forward on the tcgen05 kernel (TMA element strides)
+CONV_S2_TC = os.environ.get('TFB_CONV_S2_TC', '1') == '1'       # bf16 mode: stride-2 3x3 convs forward on the tensor-core kernel (TMA element strides)
 WGRAD_STREAM = os.environ.get('TFB_WGRAD_STREAM', '1') == '1'   # bf16 mode: weight-gradient GEMMs on a third stream (they only feed AdamW)
 BN_STATS_FUSED = os.environ.get('TFB_BN_STATS_FUSED', '1') == '1'   # bf16 mode: BatchNorm statistics out of the producing conv / GEMM epilogue
-# Weight-gradient GEMMs run on a side stream next to the critical dx chain. Measured on a B200 (profiles/r2_bench_ab_*.json): letting
-# their split-K fill all 148 SMs made the step 1.3 ms SLOWER (they starve the chain); capping their persistent grid at 64 CTAs and
-# letting the library pick tile width + split factor for THAT grid (csrc/gemm_tc.cu pick_bn) is the fastest combination (-0.5 ms).
+# Weight-gradient GEMMs run on a side stream next to the critical dx chain. Letting their split-K fill every SM starves the chain;
+# their persistent grid is capped at 64 CTAs (about half the chip) and the library picks tile width + split factor for THAT grid
+# (csrc/gemm_tc.cu pick_bn).
 WGRAD_AUTO_SPLIT = os.environ.get('TFB_WGRAD_AUTO_SPLIT', '1') == '1'
 WGRAD_MAX_CTAS = int(os.environ.get('TFB_WGRAD_MAX_CTAS', '64'))
 NARROW_DGRAD_TC = os.environ.get('TFB_NARROW_DGRAD_TC', '1') == '1'   # dgrad of 3x3 convs with < 8 output channels on the tensor cores (padded dy)
@@ -107,7 +107,7 @@ DECODER_STREAMS = os.environ.get('TFB_DECODER_STREAMS', '0') == '1'   # segmenta
 #                                                                        the upsample kernels were vectorised; off)
 BN_SE_FUSED = os.environ.get('TFB_BN_SE_FUSED', '1') == '1'     # Bottleneck conv2.bn + squeeze-excite as one autograd node (SE gradient folded into BatchNorm backward)
 ADD_LN_FUSED = os.environ.get('TFB_ADD_LN_FUSED', '1') == '1'   # GPT: residual add + dropout + the next LayerNorm in one launch
-ATTN_FUSED = os.environ.get('TFB_ATTN_FUSED', '1') == '1'       # bf16 mode: fused tcgen05 attention (csrc/attn_tc.cu), no T x T tensor in HBM
+ATTN_FUSED = os.environ.get('TFB_ATTN_FUSED', '1') == '1'       # bf16 mode: fused tensor-core attention (csrc/attn_tc.cu), no T x T tensor in HBM
 
 
 def _emit16(x, want):
@@ -381,7 +381,7 @@ def _wgrad_splits(M, N, K):
 class LinearFn(Function):
     """y[M,N] = x[M,K] @ w[N,K]^T + b (ReLU). nn.Linear (transfuser.py:498-506, 538-543) and 1x1 nn.Conv2d as a GEMM.
     bf16 mode: x is cast once (kept for backward instead of the fp32 tensor), the weight comes from the bf16 mirror, and
-    forward / dgrad / wgrad all run on the tcgen05 kernel (K-major / MN-major operand descriptors, no transposes)."""
+    forward / dgrad / wgrad all run on the tensor-core kernel (K-major / MN-major operand descriptors, no transposes)."""
 
     @staticmethod
     def forward(ctx, x, w, bias, relu, want_stats=False):
@@ -692,7 +692,7 @@ def _conv_wgrad_tc(x, g16, w, groups, stride):
                 _COL_CACHE[key] = (x, col, x._version)
         dwp = dw.view(Cout, 9 * Cig) if rows == Cout else torch.empty((rows, 9 * Cig), dtype=torch.float32, device=x.device)
         ntiles = groups * ((9 * Cig + 127) // 128)
-        splits = 0 if WGRAD_AUTO_SPLIT else max(1, min(128, (2 * 148 + ntiles - 1) // ntiles, M // 256))
+        splits = 0 if WGRAD_AUTO_SPLIT else max(1, min(128, (2 * 132 + ntiles - 1) // ntiles, M // 256))
         call('tfb_gemm_bf16_tc_wgrad_batched', Cog if groups > 1 else rows, 9 * Cig, M, g16, ldg, Cog if groups > 1 else 0, col, 9 * Cin,
              9 * Cig if groups > 1 else 0, dwp, 9 * Cig, Cog * 9 * Cig, groups, splits)
         if rows != Cout:
@@ -701,7 +701,7 @@ def _conv_wgrad_tc(x, g16, w, groups, stride):
 
 
 class Conv3x3TCFn(Function):
-    """3x3 / stride 1 conv in bf16 mode: forward and dgrad as implicit GEMMs on the tcgen05 tensor cores (csrc/conv_tc.cu:
+    """3x3 / stride 1 conv in bf16 mode: forward and dgrad as implicit GEMMs on the wgmma tensor cores (csrc/conv_tc.cu:
     TMA tap-shifted NHWC tiles, no im2col); wgrad on the fp32 direct kernel."""
 
     @staticmethod
@@ -1277,7 +1277,7 @@ class AttentionFn(Function):
                     gemm(h, w_, qkv[:, i * C:(i + 1) * C], trans_b=True, bias=b_, mode='simt')
         scale = 1.0 / (hs ** 0.5)
         if fused:
-            # one launch: scores in TMEM, softmax on the TMEM lanes, probabilities through shared memory (csrc/attn_tc.cu)
+            # one launch: scores in registers, softmax on the accumulator fragments, probabilities through shared memory (csrc/attn_tc.cu)
             y = torch.empty((B * T, C), dtype=torch.float32, device=dev)
             y16 = _emit16(y, True)                           # the output feeds the proj GEMM
             lse = torch.empty((B, nh, T), dtype=torch.float32, device=dev)

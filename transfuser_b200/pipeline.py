@@ -1,5 +1,5 @@
 """GPU input pipeline (SURVEY.md §8f rank 2): the device side of CARLA_Data.__getitem__
-(/root/reference/team_code_transfuser/data.py:103-356) for a whole batch, fed with compact inputs.
+(team_code_transfuser/data.py:103-356) for a whole batch, fed with compact inputs.
 
 The reference prepares every sample on CPU workers (numpy / OpenCV) and ships expanded tensors: fp32 RGB (1.35 MB), fp32
 LiDAR histogram + target map (0.79 MB), float depth and int64 semantics (0.45 + 0.90 MB) per sample. Here the host ships
