@@ -61,7 +61,7 @@ def test_tf32_tensor_core(shape, ta, tb):
     out = torch.full((M, N), float('nan'), device='cuda')
     gemm.gemm(a, b, out, ta, tb, bias=bias, relu=False, mode='tf32')
     assert _relerr(out, _ref(a, b, ta, tb, bias, False, 1.0, 0.0, None)) < 2e-3
-    # split-K with atomics (wgrad shape class)
+    # split-K (wgrad shape class): per-split partial tiles added in split order
     out2 = torch.full((M, N), float('nan'), device='cuda')
     gemm.gemm(a, b, out2, ta, tb, bias=bias, splits=4, mode='tf32')
     assert _relerr(out2, _ref(a, b, ta, tb, bias, False, 1.0, 0.0, None)) < 2e-3

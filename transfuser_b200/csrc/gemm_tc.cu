@@ -5,7 +5,7 @@
 // 128B-swizzled shared memory and described to the MMA by a shared-memory matrix descriptor.
 //   forward  y = x W^T      : A K-major (x[M,K]),  B K-major (W[N,K])
 //   dgrad    dx = dy W      : A K-major (dy[M,N']), B MN-major (W[N',K'] read as [k][n])
-//   wgrad    dW = dy^T x    : A MN-major (dy[M',N] read as [k][m]), B MN-major (x[M',K] read as [k][n]); split-K + atomics
+//   wgrad    dW = dy^T x    : A MN-major (dy[M',N] read as [k][m]), B MN-major (x[M',K] read as [k][n]); ordered split-K
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups (wgmma issue on rows 0-63 / 64-127 of the tile, then the
 // epilogue registers -> global), warp 8 = TMA producer. One 128 x BN output tile at a time per CTA, STAGES-deep mbarrier ring
 // between TMA and the MMAs.
@@ -379,7 +379,7 @@ int dispatch_major(int BN, int transA, int transB, int M, int N, int K, const T*
 // Tile width (and, when auto_split, the split-K factor) for a [M, N] output with `nbatch` independent batches and num_kb k-blocks.
 // The kernel is bound by the bytes each CTA pulls from L2 per k-block ((128 + BN) * 128 B against ~42 B/clk per SM), so one CTA
 // costs ~ kb_per_split * (128 + BN) plus a fixed prologue / epilogue share (kFixed, in the same unit: ~6 k-blocks of a 128 x 128
-// tile) plus, for split-K, the fp32 atomics of its 128 x BN partial tile; the persistent grid runs ceil(CTAs / SMs) waves.
+// tile) plus, for split-K, the store and reload of its 128 x BN partial tile; the persistent grid runs ceil(CTAs / SMs) waves.
 // step = 32 (K-major B) or 64 (MN-major B: whole 128-byte swizzle rows). auto_split: the number of splits that fills one wave of
 // SMs while leaving >= 4 k-blocks per CTA (weight gradients: long contraction, few output tiles).
 int pick_bn(int M, int N, int zs, int step, int num_kb = 0, bool auto_split = false, int* splits_out = nullptr) {
@@ -474,7 +474,7 @@ TFB_API int tfb_gemm_bf16_tc(int transA, int transB, int M, int N, int K, const 
 }
 
 // y[M,N] (fp32) = x[M,K] W[N,K]^T (bf16 operands) as tfb_gemm_bf16_tc(0, 1, ...), and in the same epilogue the per-column
-// statistics of y: stats[n] += sum_m y[m][n], stats[N + n] += sum_m y[m][n]^2 (fp64 atomics; the caller zeroes stats once per
+// statistics of y: stats[n] += sum_m y[m][n], stats[N + n] += sum_m y[m][n]^2 (per-CTA sums added in CTA order; the caller zeroes stats once per
 // training step). The training-mode BatchNorm behind every 1x1 conv of the RegNetY trunks (timm BatchNormAct2d) then needs no
 // statistics pass of its own (tfb_bn_fwd_stats). ldc % 4 == 0, C 16-byte aligned.
 TFB_API int tfb_gemm_bf16_tc_stats(int M, int N, int K, const void* A, int64_t lda, const void* B, int64_t ldb, float* C, int64_t ldc,
