@@ -19,58 +19,77 @@ from transfuser_b200.config import TrainConfig  # noqa: E402
 from transfuser_b200.trainer import Trainer  # noqa: E402
 
 
+def trainer(batch):
+    """A bf16-mode Trainer on cuda:0, two eager steps in, and its device batch."""
+    import numpy as np
+    dev = torch.device('cuda:0')
+    torch.cuda.set_device(dev)
+    tr = Trainer(TrainConfig(), dev, gemm_mode='bf16')
+    host = bench.make_host_batch(batch, 0, torch, np)
+    d = {k: v.to(dev) for k, v in host.items()}
+    for _ in range(2):
+        tr.step(d)
+    torch.cuda.synchronize()
+    return tr, d
+
+
+def record(step, names):
+    """(name, args) of every C-ABI call of one step() whose name is in `names`, in call order (tensors kept alive)."""
+    lib = _lib.lib()
+    calls, orig = [], lib.call
+
+    def rec(name, *args):
+        if name in names:
+            calls.append((name, args))
+        return orig(name, *args)
+    lib.call = rec
+    try:
+        step()
+    finally:
+        lib.call = orig
+    return calls
+
+
+def graph_ms(calls, replays):
+    """ms per replay of one CUDA graph holding exactly these launches, in order."""
+    call = _lib.lib().call
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        for name, c in calls:
+            call(name, *c)
+    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for name, c in calls:
+            call(name, *c)
+    for _ in range(3):
+        g.replay()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(replays):
+        g.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / replays
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('name', nargs='?', default='tfb_gemm_bf16_tc')
     ap.add_argument('--batch', type=int, default=10)
     ap.add_argument('--replays', type=int, default=20)
     a = ap.parse_args()
-    import numpy as np
-    dev = torch.device('cuda:0')
-    torch.cuda.set_device(dev)
-    tr = Trainer(TrainConfig(), dev, gemm_mode='bf16')
-    host = bench.make_host_batch(a.batch, 0, torch, np)
-    d = {k: v.to(dev) for k, v in host.items()}
-    for _ in range(2):
-        tr.step(d)
-    torch.cuda.synchronize()
-    lib = _lib.lib()
-    calls, orig = [], lib.call
-
-    def rec(name, *args):
-        if name == a.name:
-            calls.append(args)
-        return orig(name, *args)
-    lib.call = rec
-    tr.step(d)
-    torch.cuda.synchronize()
-    lib.call = orig
+    tr, d = trainer(a.batch)
+    calls = record(lambda: (tr.step(d), torch.cuda.synchronize()), {a.name})
     if not calls:
         print('no calls of', a.name)
         return
-    work = [_lib.Profiler._work(a.name, c) for c in calls]
+    work = [_lib.Profiler._work(a.name, c) for _, c in calls]
     flops, byts = sum(w[0] for w in work), sum(w[1] for w in work)
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        for c in calls:
-            orig(a.name, *c)
-    torch.cuda.current_stream().wait_stream(side)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for c in calls:
-            orig(a.name, *c)
-    for _ in range(3):
-        g.replay()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(a.replays):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / a.replays
+    ms = graph_ms(calls, a.replays)
     pk, how = bench.peaks()
     lines = ['%s: %d launches per step, %.3f ms per step in a dedicated graph, %.2f us per launch' % (a.name, len(calls), ms, 1e3 * ms / len(calls))]
     if flops > 0:

@@ -96,6 +96,48 @@ __device__ __forceinline__ void tfb_store_bf16x4(__nv_bfloat16* dst, int64_t i4,
   reinterpret_cast<uint2*>(dst)[i4] = o;
 }
 
+// The fold of every fixed-order cross-CTA sum. For each group g in [0, ngroups) of V consecutive outputs (partials at
+// part + off(g), V-aligned), the rows r in [0, nrows) with take(r) are added in row order, starting from +0 in the accumulator type
+// Acc, and emit(g, sum) receives the V sums. Rows with !take(r) are not read and count as +0: a fold that starts at +0 never
+// becomes -0, so they do not change the bits. Thread t of nthr takes groups t, t + nthr, ...; each thread loads kFoldBatch rows
+// (V * sizeof(P) bytes each, 16 with V = 16 / sizeof(P)) before it adds them, so the loads of a batch are in flight together.
+constexpr int kFoldBatch = 8;
+template <typename P, int V> struct FoldVec;
+template <> struct FoldVec<float, 1> { typedef float T; };
+template <> struct FoldVec<float, 4> { typedef float4 T; };
+template <> struct FoldVec<double, 1> { typedef double T; };
+template <> struct FoldVec<double, 2> { typedef double2 T; };
+template <typename Acc, int V, typename P, class Off, class Take, class Emit>
+__device__ __forceinline__ void ordered_fold(const P* part, int64_t row_stride, int nrows, int64_t ngroups, Off off, Take take, Emit emit,
+                                             int t, int nthr) {
+  typedef typename FoldVec<P, V>::T Vec;
+  for (int64_t g = t; g < ngroups; g += nthr) {
+    const P* p = part + off(g);
+    Acc s[V];
+#pragma unroll
+    for (int v = 0; v < V; ++v) s[v] = Acc(0);
+    for (int r0 = 0; r0 < nrows; r0 += kFoldBatch) {
+      P x[kFoldBatch][V];
+#pragma unroll
+      for (int b = 0; b < kFoldBatch; ++b) {
+        const int r = r0 + b;
+        if (r < nrows && take(r)) {
+          const Vec q = __ldcg(reinterpret_cast<const Vec*>(p + (int64_t)r * row_stride));
+          memcpy(x[b], &q, sizeof(Vec));
+        } else {
+#pragma unroll
+          for (int v = 0; v < V; ++v) x[b][v] = P(0);
+        }
+      }
+#pragma unroll
+      for (int b = 0; b < kFoldBatch; ++b)
+#pragma unroll
+        for (int v = 0; v < V; ++v) s[v] += (Acc)x[b][v];
+    }
+    emit(g, s);
+  }
+}
+
 // Cross-block sums that give the same bits on every run. Every output index i in [0, n_out) gets exactly one contribution from
 // each split s in [0, nsplit) (ordered_store); the last block of the grid to finish (ordered_finish, called by every thread of
 // every block) adds, for each i, the contributions in split order to out[i]. part / cnt: nsplit * n_out floats and one counter
@@ -107,6 +149,20 @@ struct OrderedSum {
   int64_t n_out;
 };
 static __device__ __forceinline__ void ordered_store(const OrderedSum& o, int split, int64_t i, float v) { o.part[(int64_t)split * o.n_out + i] = v; }
+// out[i] (+)= the fold of part[0..nsplit)[i] for i in [0, n_out), by thread t of nthr; 16-byte loads when n_out % 4 == 0.
+static __device__ __forceinline__ void ordered_sum_range(const float* part, int nsplit, int64_t n_out, float* out, bool assign, int t, int nthr) {
+  auto all = [](int) { return true; };
+  if (n_out % 4 == 0 && (reinterpret_cast<uintptr_t>(part) & 15) == 0) {
+    ordered_fold<float, 4>(part, n_out, nsplit, n_out / 4, [](int64_t g) { return g * 4; }, all, [&](int64_t g, const float (&s)[4]) {
+#pragma unroll
+      for (int v = 0; v < 4; ++v) out[g * 4 + v] = (assign ? 0.f : out[g * 4 + v]) + s[v];
+    }, t, nthr);
+  } else {
+    ordered_fold<float, 1>(part, n_out, nsplit, n_out, [](int64_t g) { return g; }, all, [&](int64_t g, const float (&s)[1]) {
+      out[g] = (assign ? 0.f : out[g]) + s[0];
+    }, t, nthr);
+  }
+}
 static __device__ __forceinline__ void ordered_finish(const OrderedSum& o, float* out) {
   if (!o.cnt) return;                 // summed by ordered_sum_kernel after the launch instead (large n_out)
   __shared__ bool last;
@@ -117,21 +173,14 @@ static __device__ __forceinline__ void ordered_finish(const OrderedSum& o, float
   __syncthreads();
   if (!last) return;
   __threadfence();
-  for (int64_t i = tid; i < o.n_out; i += nthr) {
-    float s = 0.f;
-    for (int k = 0; k < o.nsplit; ++k) s += __ldcg(o.part + (int64_t)k * o.n_out + i);
-    out[i] += s;
-  }
+  ordered_sum_range(o.part, o.nsplit, o.n_out, out, false, tid, nthr);
   if (tid == 0) *o.cnt = 0u;
 }
-// out[i] += sum over splits k (in order) of part[k][i], one thread per output: the last step of an OrderedSum whose n_out is too
-// large for one CTA (launched after the kernel that stored the partials, with o.cnt = nullptr there).
-static __global__ void __launch_bounds__(256) ordered_sum_kernel(const float* __restrict__ part, int nsplit, int64_t n_out, float* __restrict__ out) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_out; i += (int64_t)gridDim.x * blockDim.x) {
-    float s = 0.f;
-    for (int k = 0; k < nsplit; ++k) s += part[(int64_t)k * n_out + i];
-    out[i] += s;
-  }
+// out[i] += sum over splits k (in order) of part[k][i] (assign: out[i] = +0 + that sum): the last step of an OrderedSum whose n_out
+// is too large for one CTA (launched after the kernel that stored the partials, with o.cnt = nullptr there).
+static __global__ void __launch_bounds__(256) ordered_sum_kernel(const float* __restrict__ part, int nsplit, int64_t n_out, float* __restrict__ out,
+                                                                 bool assign = false) {
+  ordered_sum_range(part, nsplit, n_out, out, assign, (int)(blockIdx.x * blockDim.x + threadIdx.x), (int)(gridDim.x * blockDim.x));
 }
 
 static inline int ordered_alloc(OrderedSum& o, int nsplit, int64_t n_out, cudaStream_t s) {

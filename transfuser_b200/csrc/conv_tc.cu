@@ -143,7 +143,9 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_consta
         }
       }
     }
-    if (stats) tc::stat_flush(s_stat, stats, Cout, (int)threadIdx.x, ws, ws_cnt);
+    if (stats)    // tile t lies in channel block t % gblocks
+      tc::stat_flush(s_stat, stats, Cout, (int)threadIdx.x, ws, ws_cnt, total_tiles, total_tiles / gblocks, [=](int t) { return t % gblocks; },
+                     [=](int g, int i) { return g + i * gblocks; }, [=](int g) { return make_int2(g * nb_real, min(nb_real, Cout - g * nb_real)); });
   }
 }
 
@@ -186,9 +188,10 @@ int launch_conv(const void* x16, const void* wpack, const float* bias, float* y,
   const int per_sm = (SMEM <= 110 * 1024) ? 2 : 1;
   const int64_t cap = (int64_t)tfb_num_sms() * per_sm;
   const int grid = (int)(total < cap ? total : cap);
-  TfbScratch wk;                 // the CTAs' statistics, reduced in CTA order by the last one
+  TfbScratch wk;                 // the CTAs' statistics and one arrival counter per channel block (tc::stat_flush)
   if (stats) {
-    const int rc = tfb_scratch(wk, (size_t)grid * 2 * Cy, 1, stream);
+    TFB_REQUIRE(grid <= tc::kMaxStatGrid);
+    const int rc = tfb_scratch(wk, (size_t)grid * 2 * Cy, (size_t)gblocks, stream);
     if (rc != TFB_OK) return rc;
   }
   kern<<<grid, kThreads, SMEM, stream>>>(mx, mw, y, bias, H, W, Cy, tiles_w, tiles_h, c_step, nchunks, nb_real, relu, gblocks, (int)total, stride, stats,

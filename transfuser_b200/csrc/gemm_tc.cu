@@ -43,8 +43,9 @@ constexpr int kMaxBN = 192;
 constexpr int kThreads = 288;                                 // warps 0-7: two consumer warpgroups; warp 8: TMA producer
 constexpr int kStageFloats = 16 * 36;                         // one warp's epilogue staging block (16 rows, padded stride 36)
 constexpr int kABytes = BM * 128;
-constexpr int kSmemMax = 232448 - 64;                         // 227 KB opt-in limit, less the kernel's static shared flags
+constexpr int kSmemMax = 232448 - 256;                        // 227 KB opt-in limit, less the kernel's static shared memory (flags)
 constexpr int kSmemFixed = 256 + 8 * kStageFloats * 4 + 1024; // barriers + epilogue staging + alignment slack
+constexpr int64_t kPostFoldBytes = 256 * 1024;                // split-K partials one CTA folds at most (see launch_bn)
 
 template <typename T, bool A_MN, bool B_MN, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -167,7 +168,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       const bool add_bias = bias != nullptr && sz == 0;
       if (splits > 1) {
         // split-K: the partial tile goes to its own slice of the workspace; the last split of the tile to arrive adds the slices
-        // to C in split order (the same bits every run, whatever order the CTAs run in)
+        // to C in split order (the same bits every run, whatever order the CTAs run in). ws_cnt == nullptr: the slices are added by
+        // ordered_sum_kernel after the launch instead.
         __shared__ unsigned int s_last;
         float* part = ws + (int64_t)(bz * splits + sz) * M * N;
 #pragma unroll
@@ -175,6 +177,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           const int m = m0 + wg * 64 + tc::frag_row(t128, i), n = n0 + tc::frag_col(t128, i);
           if (m < M && n < N) part[(int64_t)m * N + n] = alpha * acc[i] + (add_bias ? bias[n] : 0.f);
         }
+        if (!ws_cnt) continue;
         __threadfence();
         asm volatile("bar.sync 1, %0;" ::"n"(tc::kConsumers) : "memory");
         const int tile = (m0 / BM) + tiles_m * ((n0 / BN) + tiles_n * bz);
@@ -183,13 +186,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         if (s_last) {
           __threadfence();
           if (threadIdx.x == 0) ws_cnt[tile] = 0u;   // the stream's scratch counters are zero on entry
-          for (int e = threadIdx.x; e < BM * BN; e += tc::kConsumers) {
-            const int m = m0 + e / BN, n = n0 + e % BN;
-            if (m < M && n < N) {
-              float s = 0.f;
-              for (int z = 0; z < splits; ++z) s += __ldcg(ws + ((int64_t)(bz * splits + z) * M + m) * N + n);
-              Cbase[(int64_t)bz * c_bstride + (int64_t)m * ldc + n] += s;
-            }
+          // C = +0 + sum (beta == 0: C is not read) or C + sum (beta == 1)
+          const int rows = min(BM, M - m0), cols = min(BN, N - n0);
+          const float* p0 = ws + (int64_t)bz * splits * M * N + (int64_t)m0 * N + n0;
+          float* c0 = Cbase + (int64_t)bz * c_bstride + (int64_t)m0 * ldc + n0;
+          const bool assign = beta == 0.f;
+          auto all = [](int) { return true; };
+          if ((N & 3) == 0) {            // then cols % 4 == 0 and every slice is 16-byte aligned
+            const int cq = cols / 4;
+            ordered_fold<float, 4>(p0, (int64_t)M * N, splits, (int64_t)rows * cq, [&](int64_t g) { return (g / cq) * N + (g % cq) * 4; }, all,
+                                       [&](int64_t g, const float (&sum)[4]) {
+                                         float* o = c0 + (g / cq) * ldc + (g % cq) * 4;
+#pragma unroll
+                                         for (int v = 0; v < 4; ++v) o[v] = (assign ? 0.f : o[v]) + sum[v];
+                                       }, (int)threadIdx.x, tc::kConsumers);
+          } else {
+            ordered_fold<float, 1>(p0, (int64_t)M * N, splits, (int64_t)rows * cols, [&](int64_t g) { return (g / cols) * N + g % cols; }, all,
+                                       [&](int64_t g, const float (&sum)[1]) {
+                                         float* o = c0 + (g / cols) * ldc + g % cols;
+                                         *o = (assign ? 0.f : *o) + sum[0];
+                                       }, (int)threadIdx.x, tc::kConsumers);
           }
         }
         continue;
@@ -232,7 +248,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         }
       }
     }
-    if (stats) tc::stat_flush(s_stat, stats, N, (int)threadIdx.x, ws, ws_cnt);
+    if (stats)    // stats: one batch, one split, so tile t lies in column block t / tiles_m
+      tc::stat_flush(s_stat, stats, N, (int)threadIdx.x, ws, ws_cnt, total_tiles, tiles_m, [=](int t) { return t / tiles_m; },
+                     [=](int g, int i) { return g * tiles_m + i; }, [=](int g) { return make_int2(g * BN, min(BN, N - g * BN)); });
   }
 }
 
@@ -303,17 +321,9 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
   // reduction epilogue adds into C with coalesced vector reductions instead of the scalar read-modify-write path
   const bool accumulate = beta == 1.f && !relu && !stats && !C16 && nbatch == 1;
   const int atomic_out = (splits > 1 || accumulate) ? 1 : 0;
-  if (atomic_out) {
+  if (atomic_out) {   // split-K with beta == 0 stores +0 + sum into C, so C is not cleared first
     if (relu) { tfb_set_last_error("split-K cannot fuse ReLU"); return TFB_ERR_ARG; }
-    if (beta == 0.f) {
-      if (ldc == N && (nbatch == 1 || c_bstride == (int64_t)M * N)) {   // outputs are one contiguous block: a single memset
-        if (cudaMemsetAsync(C, 0, (size_t)nbatch * M * N * sizeof(float), stream) != cudaSuccess) return TFB_ERR_DRIVER;
-      } else {
-        for (int b = 0; b < nbatch; ++b)
-          if (cudaMemset2DAsync(C + (int64_t)b * c_bstride, ldc * sizeof(float), 0, (size_t)N * sizeof(float), M, stream) != cudaSuccess)
-            return TFB_ERR_DRIVER;
-      }
-    } else if (beta != 1.f) { tfb_set_last_error("split-K needs beta in {0,1}"); return TFB_ERR_ARG; }
+    if (beta != 0.f && beta != 1.f) { tfb_set_last_error("split-K needs beta in {0,1}"); return TFB_ERR_ARG; }
   }
   auto kern = gemm_tc_kernel<T, A_MN, B_MN, BN>;
   static bool attr_done = false;
@@ -330,17 +340,27 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
   int grid = (int)(total < tfb_num_sms() ? total : tfb_num_sms());
   if (g_max_ctas > 0 && grid > g_max_ctas) grid = g_max_ctas;
   // workspace of the ordered cross-CTA reductions: split-K partial tiles + one counter per output tile, or the CTAs' statistics
+  // A tile's split-K fold is one CTA's work. When that is large (few output tiles, many splits: the weight gradients of the narrow
+  // early layers), all slices are added after the kernel by a grid-wide ordered_sum_kernel instead (same order, same bits).
+  const bool post_fold = splits > 1 && nbatch == 1 && ldc == N && (int64_t)splits * (M < BM ? M : BM) * (N < BN ? N : BN) * 4 > kPostFoldBytes;
   TfbScratch ws;
   if (splits > 1) {
     const int rc = tfb_scratch(ws, (size_t)nbatch * splits * M * N, (size_t)tiles_m * tiles_n * nbatch, stream);
     if (rc != TFB_OK) return rc;
   } else if (stats) {
-    const int rc = tfb_scratch(ws, (size_t)grid * 2 * N, 1, stream);
+    TFB_REQUIRE(grid <= tc::kMaxStatGrid);
+    const int rc = tfb_scratch(ws, (size_t)grid * 2 * N, (size_t)tiles_n, stream);
     if (rc != TFB_OK) return rc;
   }
   kern<<<grid, kThreads, smem_total, stream>>>(ma, mb, C, ldc, M, N, num_kb, kb_per_split, bias, alpha, beta, relu, atomic_out, splits,
-                                               a_step, b_step, c_bstride, tiles_m, tiles_n, (int)total, stages, stats, C16, ws.f, ws.cnt);
+                                               a_step, b_step, c_bstride, tiles_m, tiles_n, (int)total, stages, stats, C16, ws.f,
+                                               post_fold ? nullptr : ws.cnt);
   TFB_CHECK_LAUNCH();
+  if (post_fold) {
+    const int64_t n_out = (int64_t)M * N, groups = n_out % 4 == 0 ? n_out / 4 : n_out;
+    ordered_sum_kernel<<<tfb_grid(groups, 64), 64, 0, stream>>>(ws.f, splits, n_out, C, beta == 0.f);
+    TFB_CHECK_LAUNCH();
+  }
   return TFB_OK;
 }
 

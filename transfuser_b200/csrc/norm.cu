@@ -26,30 +26,41 @@ struct Finalize {
   float* running_var;
   float* zero_buf;       // optional: zero_n floats cleared by the last block (the SE pooling accumulator of the NEXT kernel on the
   int zero_n;            // stream, tfb_bn_fwd with pooling: saves the memset node)
-  double* part;          // [nsplit][nsums]: each row split's partial sums; the last block adds them in split order, so the result is
-                         // the same bits on every run (set by the launcher, see with_partials)
+  double* part;          // [nsplit][nsums]: each row split's partial sums; the last block of a slab adds them in split order, so the
+                         // result is the same bits on every run (set by the launcher, see alloc_partials)
+  unsigned int* cnt;     // one arrival counter per channel slab, in the stream's scratch (alloc_partials)
 };
 
-__device__ __forceinline__ void finalize_last_block(double* sums, int C, const Finalize& f, int nsplit) {
+// The partials of channel slab `slab` (channels [slab * slab_w, +slab_w)) come from the nsplit blocks of that slab; the last of them
+// to arrive (arrival counter f.cnt[slab]) folds the slab's channels in split order and finalises them, so the slabs finish in parallel.
+// MAXW >= slab_w: 32 or 128 for the slabs of the 2-D grids, 512 for colreduce_flat_kernel (all channels, C / 4 <= 128).
+template <int MAXW>
+__device__ __forceinline__ void finalize_last_block(double* sums, int C, const Finalize& f, int nsplit, int slab, int slab_w) {
   if (f.kind == 0) return;
   __shared__ bool is_last;
+  __shared__ double fs[2][MAXW];
   __threadfence();
   __syncthreads();
   const int tid = threadIdx.y * blockDim.x + threadIdx.x, nthr = blockDim.x * blockDim.y;
-  if (tid == 0) {
-    unsigned int* counter = reinterpret_cast<unsigned int*>(sums + f.nsums);
-    const unsigned int ticket = atomicAdd(counter, 1u);
-    is_last = ticket == gridDim.x * gridDim.y * gridDim.z - 1;
-  }
+  if (tid == 0) is_last = atomicAdd(f.cnt + slab, 1u) == (unsigned int)(nsplit - 1);
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  for (int c = tid; c < C; c += nthr) {
-    double s0 = 0.0, s1 = 0.0;
-    for (int j = 0; j < nsplit; ++j) {
-      s0 += __ldcg(f.part + (int64_t)j * f.nsums + c);
-      if (f.nsums > C) s1 += __ldcg(f.part + (int64_t)j * f.nsums + C + c);
-    }
+  const int lo = slab * slab_w, w = min(slab_w, C - lo), nq = f.nsums > C ? 2 : 1;
+  auto all = [](int) { return true; };
+  if ((C & 1) == 0) {                // then lo and w are even: pairs of channels, 16-byte loads
+    const int hw = w / 2;
+    ordered_fold<double, 2>(f.part, f.nsums, nsplit, (int64_t)nq * hw, [&](int64_t g) { return (g / hw) * C + lo + (g % hw) * 2; }, all,
+                            [&](int64_t g, const double (&s)[2]) { fs[g / hw][(g % hw) * 2] = s[0]; fs[g / hw][(g % hw) * 2 + 1] = s[1]; },
+                            tid, nthr);
+  } else {
+    ordered_fold<double, 1>(f.part, f.nsums, nsplit, (int64_t)nq * w, [&](int64_t g) { return (g / w) * C + lo + g % w; }, all,
+                            [&](int64_t g, const double (&s)[1]) { fs[g / w][g % w] = s[0]; }, tid, nthr);
+  }
+  __syncthreads();
+  for (int i = tid; i < w; i += nthr) {
+    const int c = lo + i;
+    const double s0 = fs[0][i], s1 = nq > 1 ? fs[1][i] : 0.0;
     if (f.kind == 1) {
       const double mean = s0 / (double)f.M;
       double var = s1 / (double)f.M - mean * mean;
@@ -70,8 +81,9 @@ __device__ __forceinline__ void finalize_last_block(double* sums, int C, const F
     sums[c] = 0.0;
     if (f.nsums > C) sums[C + c] = 0.0;
   }
-  for (int i = tid; i < f.zero_n; i += nthr) f.zero_buf[i] = 0.f;
-  if (tid == 0) *reinterpret_cast<unsigned int*>(sums + f.nsums) = 0u;
+  if (slab == 0)
+    for (int i = tid; i < f.zero_n; i += nthr) f.zero_buf[i] = 0.f;
+  if (tid == 0) f.cnt[slab] = 0u;    // the stream's scratch counters are zero on entry
 }
 
 // Gradient entering a BatchNorm whose output feeds a squeeze-excite gate (y = bn_out * gate[n][c]): with dy the gradient of the SE
@@ -125,7 +137,7 @@ colreduce_kernel(const float* __restrict__ x, int64_t ldx, const float* __restri
     fin.part[(int64_t)blockIdx.y * fin.nsums + c] = t0;
     if (fin.nsums > C) fin.part[(int64_t)blockIdx.y * fin.nsums + C + c] = t1;
   }
-  finalize_last_block(out, C, fin, gridDim.y);
+  finalize_last_block<32>(out, C, fin, gridDim.y, blockIdx.x, 32);
 }
 
 // float4 variant (C % 4 == 0, 16-byte aligned rows): threadIdx.x -> one channel QUAD inside a 128-channel slab, two rows in
@@ -207,7 +219,7 @@ colreduce4_kernel(const float* __restrict__ x, int64_t ldx, const float* __restr
     if (tv < 4) fin.part[(int64_t)blockIdx.y * fin.nsums + cc + tv] = t;
     else if (fin.nsums > C) fin.part[(int64_t)blockIdx.y * fin.nsums + C + cc + tv - 4] = t;
   }
-  finalize_last_block(out, C, fin, gridDim.y);
+  finalize_last_block<128>(out, C, fin, gridDim.y, blockIdx.x, 128);
 }
 
 // Narrow matrices (C / 4 <= 128 channel quads: the 32-, 72- and 216-channel maps of the stem / stage 1 / stage 2, i.e. the LARGEST
@@ -279,7 +291,7 @@ colreduce_flat_kernel(const float* __restrict__ x, const float* __restrict__ dy,
     if (v < 4) fin.part[(int64_t)blockIdx.x * fin.nsums + qq * 4 + v] = sum;
     else if (fin.nsums > C) fin.part[(int64_t)blockIdx.x * fin.nsums + C + qq * 4 + v - 4] = sum;
   }
-  finalize_last_block(out, C, fin, gridDim.x);
+  finalize_last_block<512>(out, C, fin, gridDim.x, 0, C);
 }
 
 // y = (x - mean) * invstd * gamma + beta (ReLU); 4 channels per thread (C % 4 == 0).
@@ -670,7 +682,7 @@ ln_bwd_param_kernel(const float* __restrict__ x, const float* __restrict__ dy, i
     fin.part[(int64_t)blockIdx.y * fin.nsums + c] = (double)tb;
     fin.part[(int64_t)blockIdx.y * fin.nsums + C + c] = (double)ta;
   }
-  finalize_last_block(sums, C, fin, gridDim.y);
+  finalize_last_block<32>(sums, C, fin, gridDim.y, blockIdx.x, 32);
 }
 
 // Backward prologue of a dense layer, one pass over dy [M, C]:  g = relu ? dy * (y > 0) : dy;  optional outputs: g in fp32, g in
@@ -700,7 +712,7 @@ grad_prep_kernel(const float* __restrict__ dy, const float* __restrict__ y, floa
       for (int j = 0; j < 8; ++j) t += sm[j][threadIdx.x];
       fin.part[(int64_t)blockIdx.y * fin.nsums + c] = (double)t;
     }
-    finalize_last_block(sums, C, fin, gridDim.y);
+    finalize_last_block<32>(sums, C, fin, gridDim.y, blockIdx.x, 32);
   }
 }
 
@@ -723,11 +735,12 @@ __global__ void __launch_bounds__(256) scale_gate_kernel(const float* __restrict
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// fin.part for a reduction with nsplit row splits, in the stream's scratch.
-int alloc_partials(Finalize& fin, int64_t nsplit, cudaStream_t stream) {
+// fin.part for a reduction with nsplit row splits and fin.cnt for `slabs` channel slabs, in the stream's scratch.
+int alloc_partials(Finalize& fin, int64_t nsplit, int slabs, cudaStream_t stream) {
   TfbScratch w;
-  const int rc = tfb_scratch(w, (size_t)(2 * nsplit * fin.nsums), 0, stream);   // doubles = 2 floats each
+  const int rc = tfb_scratch(w, (size_t)(2 * nsplit * fin.nsums), (size_t)slabs, stream);   // doubles = 2 floats each
   fin.part = reinterpret_cast<double*>(w.f);
+  fin.cnt = w.cnt;
   return rc;
 }
 
@@ -760,17 +773,17 @@ int launch_colreduce(const float* x, int64_t ldx, const float* dy, int64_t M, in
     const int64_t cap = (int64_t)tfb_num_sms() * 4;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    if ((rc = alloc_partials(fin, blocks, stream)) != TFB_OK) return rc;
+    if ((rc = alloc_partials(fin, blocks, 1, stream)) != TFB_OK) return rc;
     colreduce_flat_kernel<MODE><<<(int)blocks, 256, 0, stream>>>(x, dy, M, C, out, mean, invstd, gamma, beta, relu, ymask, fin);
   } else if (vec) {
     const int slabs = (C / 4 + 31) / 32;
     dim3 grid(slabs, colreduce_splits(M, slabs));
-    if ((rc = alloc_partials(fin, grid.y, stream)) != TFB_OK) return rc;
+    if ((rc = alloc_partials(fin, grid.y, grid.x, stream)) != TFB_OK) return rc;
     colreduce4_kernel<MODE><<<grid, block, 0, stream>>>(x, ldx, dy, M, C, out, mean, invstd, gamma, beta, relu, ymask, fin);
   } else {
     const int slabs = (C + 31) / 32;
     dim3 grid(slabs, colreduce_splits(M, slabs));
-    if ((rc = alloc_partials(fin, grid.y, stream)) != TFB_OK) return rc;
+    if ((rc = alloc_partials(fin, grid.y, grid.x, stream)) != TFB_OK) return rc;
     colreduce_kernel<MODE><<<grid, block, 0, stream>>>(x, ldx, dy, M, C, out, mean, invstd, gamma, beta, relu, ymask, fin);
   }
   TFB_CHECK_LAUNCH();
@@ -890,13 +903,13 @@ static int bn_bwd_impl(const float* x, const float* dy, float* dx, int64_t M, in
       const int64_t cap = (int64_t)tfb_num_sms() * 4;
       if (blocks > cap) blocks = cap;
       if (blocks < 1) blocks = 1;
-      if ((rc = alloc_partials(fin, blocks, stream)) != TFB_OK) return rc;
+      if ((rc = alloc_partials(fin, blocks, 1, stream)) != TFB_OK) return rc;
       colreduce_flat_kernel<1><<<(int)blocks, 256, 0, stream>>>(x, dy, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu, ymask, fin,
                                                                se_gate, se_dpool, hw);
     } else {
       const int slabs = (C / 4 + 31) / 32;
       dim3 grid(slabs, colreduce_splits(M, slabs)), block(32, 8);
-      if ((rc = alloc_partials(fin, grid.y, stream)) != TFB_OK) return rc;
+      if ((rc = alloc_partials(fin, grid.y, grid.x, stream)) != TFB_OK) return rc;
       colreduce4_kernel<1><<<grid, block, 0, stream>>>(x, C, dy, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu, ymask, fin, se_gate,
                                                        se_dpool, hw);
     }
@@ -956,7 +969,7 @@ TFB_API int tfb_grad_prep(const float* dy, const float* y, float* g32, void* g16
   dim3 grid(slabs, colreduce_splits(M, slabs)), block(32, 8);
   Finalize fin = {dbias ? 3 : 0, C, M, 0.f, 0.f, dbias, nullptr, nullptr, nullptr};
   if (dbias) {
-    const int rc = alloc_partials(fin, grid.y, stream);
+    const int rc = alloc_partials(fin, grid.y, grid.x, stream);
     if (rc != TFB_OK) return rc;
   }
   grad_prep_kernel<<<grid, block, 0, stream>>>(dy, y, g32, (__nv_bfloat16*)g16_bf16, dbias ? sums_ws : nullptr, M, C, fin);
@@ -985,7 +998,7 @@ TFB_API int tfb_layernorm_bwd(const float* x, const float* dy, float* dx, int64_
   if (splits < 1) splits = 1;
   dim3 grid(slabs, splits), block(32, 8);
   Finalize fin = {2, 2 * C, R, 0.f, 0.f, dbeta, dgamma, nullptr, nullptr};
-  const int rc = alloc_partials(fin, grid.y, stream);
+  const int rc = alloc_partials(fin, grid.y, grid.x, stream);
   if (rc != TFB_OK) return rc;
   ln_bwd_param_kernel<<<grid, block, 0, stream>>>(x, dy, R, C, save_mean, save_rstd, sums_ws, fin);
   TFB_CHECK_LAUNCH();
@@ -1019,7 +1032,7 @@ TFB_API int tfb_add_dropout_ln_bwd(const float* xnew, const float* dh, const flo
   if (splits < 1) splits = 1;
   dim3 grid(slabs, splits), block(32, 8);
   Finalize fin = {2, 2 * C, R, 0.f, 0.f, dbeta, dgamma, nullptr, nullptr};
-  const int rc = alloc_partials(fin, grid.y, stream);
+  const int rc = alloc_partials(fin, grid.y, grid.x, stream);
   if (rc != TFB_OK) return rc;
   ln_bwd_param_kernel<<<grid, block, 0, stream>>>(xnew, dh, R, C, save_mean, save_rstd, sums_ws, fin);
   TFB_CHECK_LAUNCH();

@@ -7,6 +7,7 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include "common.cuh"
 #include "wgmma.cuh"
 
 namespace tc {
@@ -201,22 +202,49 @@ __device__ __forceinline__ void stat_fold(float* s_stat, const float* wstat, int
   }
   asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
 }
-__device__ __forceinline__ void stat_flush(const float* s_stat, double* stats, int n, int t, float* ws, unsigned int* cnt) {
-  __shared__ unsigned int s_last;
+// The columns form blocks (a GEMM tile's columns, a conv tile's channel block) and each of the `total` tiles of the persistent grid
+// (tile = blockIdx.x + k * gridDim.x) lies in one block: blk(tile). Block g has tpb tiles, tile(g, i) for i < tpb, and the
+// columns [cols(g).x, cols(g).x + cols(g).y). cnt holds one counter per block: each CTA adds one per tile it ran, and the CTA that
+// brings block g's counter to tpb folds block g's columns over the CTAs that ran one of its tiles, in CTA order (the other CTAs'
+// rows are +0 for these columns and are skipped). So the folds of different blocks run in different CTAs, in parallel.
+constexpr int kMaxStatGrid = 1024;
+template <class Blk, class Tile, class Cols>
+__device__ __forceinline__ void stat_flush(const float* s_stat, double* stats, int n, int t, float* ws, unsigned int* cnt, int total, int tpb,
+                                           Blk blk, Tile tile, Cols cols) {
+  __shared__ unsigned int s_last[2], s_contrib[kMaxStatGrid / 32];   // s_last by tile parity: written again only two barriers later
   asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
   for (int i = t; i < 2 * n; i += kConsumers) ws[(int64_t)blockIdx.x * 2 * n + i] = s_stat[i];
   __threadfence();
   asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
-  if (t == 0) s_last = atomicAdd(cnt, 1u) == gridDim.x - 1;
-  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
-  if (!s_last) return;
-  __threadfence();
-  for (int i = t; i < 2 * n; i += kConsumers) {
-    double s = 0.0;
-    for (unsigned int b = 0; b < gridDim.x; ++b) s += (double)__ldcg(ws + (int64_t)b * 2 * n + i);
-    stats[i] += s;
+  for (int k = blockIdx.x, p = 0; k < total; k += gridDim.x, p ^= 1) {
+    const int g = blk(k);
+    if (t == 0) s_last[p] = atomicAdd(cnt + g, 1u) == (unsigned int)(tpb - 1);
+    for (int w = t; w < kMaxStatGrid / 32; w += kConsumers) s_contrib[w] = 0u;
+    asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+    if (!s_last[p]) continue;        // block-uniform
+    __threadfence();
+    for (int i = t; i < tpb; i += kConsumers) {
+      const int b = tile(g, i) % gridDim.x;
+      atomicOr(&s_contrib[b >> 5], 1u << (b & 31));
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+    const int2 c = cols(g);
+    auto take = [&](int b) { return (s_contrib[b >> 5] >> (b & 31)) & 1u; };
+    if ((n & 3) == 0) {              // then c.x and c.y are multiples of 4 too
+      const int gq = c.y / 4;
+      ordered_fold<double, 4>(ws, 2 * n, (int)gridDim.x, 2 * gq, [&](int64_t j) { return (int64_t)(j / gq) * n + c.x + (j % gq) * 4; }, take,
+                              [&](int64_t j, const double (&s)[4]) {
+                                double* o = stats + (j / gq) * n + c.x + (j % gq) * 4;
+#pragma unroll
+                                for (int v = 0; v < 4; ++v) o[v] += s[v];
+                              }, t, kConsumers);
+    } else {
+      ordered_fold<double, 1>(ws, 2 * n, (int)gridDim.x, 2 * c.y, [&](int64_t j) { return (int64_t)(j / c.y) * n + c.x + j % c.y; }, take,
+                              [&](int64_t j, const double (&s)[1]) { stats[(j / c.y) * n + c.x + j % c.y] += s[0]; }, t, kConsumers);
+    }
+    if (t == 0) cnt[g] = 0u;         // the stream's scratch counters are zero on entry
+    asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
   }
-  if (t == 0) *cnt = 0u;               // the stream's scratch counters are zero on entry
 }
 
 // ---------------- descriptors ----------------
