@@ -7,13 +7,24 @@ load unchanged. The nn.Conv2d / nn.BatchNorm2d / nn.Linear / nn.LayerNorm object
 their forward is never called — every op runs through transfuser_b200.ops (hand-written sm_90a kernels, NHWC inside).
 
 The RegNetY-3.2GF definition (timm 0.5.4 `regnety_032`: stem 32, widths 72/216/576/1512, depths 2/5/13/1, group width 24,
-SE ratio 0.25) is restated from timm's published config; timm itself is not a dependency."""
+SE ratio 0.25) and the BasicBlock ResNets (timm 0.5.4 `resnet18` / `resnet34`: 7x7 stem and 3x3 max-pool, widths 64/128/256/512,
+depths 2/2/2/2 and 3/4/6/3) are restated from timm's published definitions; timm itself is not a dependency."""
 import torch
 from torch import nn
 
 from . import ops
 
 REGNETY_032 = dict(stem_width=32, widths=(72, 216, 576, 1512), depths=(2, 5, 13, 1), group_w=24, se_ratio=0.25)
+RESNET_DEPTHS = {'resnet18': (2, 2, 2, 2), 'resnet34': (3, 4, 6, 3)}
+RESNET_WIDTHS = (64, 128, 256, 512)
+
+
+def _conv_bn(conv, bn, x, stride=1, groups=1, act=True, emit16=False, residual=None, pool=False):
+    """bn(conv(x)) with the ReLU (act), the residual add and the SE pool fused into the BatchNorm passes (see _ConvBn.run)."""
+    y = ops.conv2d(x, conv.weight, None, stride, groups, bn_stats=bn.training)
+    # bwd16: this conv has no bias / ReLU of its own, so BatchNorm's dx is exactly the dy its tensor-core dgrad / wgrad read
+    return ops.batch_norm(y, bn, act or residual is not None, bn.training, emit16, bwd16=conv.in_channels % 8 == 0, residual=residual,
+                          pool=pool)
 
 
 class _ConvBn(nn.Module):
@@ -28,10 +39,7 @@ class _ConvBn(nn.Module):
     def run(self, x, emit16=False, residual=None, pool=False):
         """emit16: the output is the operand of a tensor-core GEMM / conv next (bf16 mode: BatchNorm writes its bf16 copy too).
         residual: relu(bn(conv(x)) + residual) — the Bottleneck tail, add and ReLU fused into the BatchNorm passes."""
-        y = ops.conv2d(x, self.conv.weight, None, self.stride, self.groups, bn_stats=self.bn.training)
-        # bwd16: this conv has no bias / ReLU of its own, so BatchNorm's dx is exactly the dy its tensor-core dgrad / wgrad read
-        return ops.batch_norm(y, self.bn, self.act or residual is not None, self.bn.training, emit16,
-                              bwd16=self.conv.in_channels % 8 == 0, residual=residual, pool=pool)
+        return _conv_bn(self.conv, self.bn, x, self.stride, self.groups, self.act, emit16, residual, pool)
 
 
 class _SE(nn.Module):
@@ -69,11 +77,8 @@ class _Bottleneck(nn.Module):
         return self.conv3.run(y, emit16=emit16, residual=sc)      # relu(conv3.bn(conv3(y)) + shortcut)
 
 
-class _Stage(nn.Module):
-    def __init__(self, cin, cout, depth, group_w, se_ratio):
-        super().__init__()
-        for i in range(depth):
-            self.add_module('b%d' % (i + 1), _Bottleneck(cin if i == 0 else cout, cout, 2 if i == 0 else 1, group_w, se_ratio))
+class _Blocks(nn.Module):
+    """A trunk stage: its children are the residual blocks, run in registration order."""
 
     def run(self, x, last16=True):
         """last16 = False when the stage output goes to a GPT fusion (token pooling / upsample-add), not straight into a conv."""
@@ -81,6 +86,13 @@ class _Stage(nn.Module):
         for i, blk in enumerate(blocks):
             x = blk.run(x, emit16=last16 or i + 1 < len(blocks))
         return x
+
+
+class _Stage(_Blocks):
+    def __init__(self, cin, cout, depth, group_w, se_ratio):
+        super().__init__()
+        for i in range(depth):
+            self.add_module('b%d' % (i + 1), _Bottleneck(cin if i == 0 else cout, cout, 2 if i == 0 else 1, group_w, se_ratio))
 
 
 class _RegNet(nn.Module):
@@ -103,33 +115,132 @@ class _RegNet(nn.Module):
                 if m.bias is not None:
                     nn.init.zeros_(m.bias)
 
+    @property
+    def stages(self):
+        return self.s1, self.s2, self.s3, self.s4
+
+    def run_stem(self, x):
+        """The encoders alias `conv1` / `bn1` to the stem (the LiDAR encoders replace `conv1`, transfuser.py:446-453); a trunk
+        used whole (late fusion) runs `stem` itself."""
+        conv, bn = (self.conv1, self.bn1) if 'conv1' in self._modules else (self.stem.conv, self.stem.bn)
+        return _conv_bn(conv, bn, x, stride=2, emit16=True)
+
+
+class _BasicBlock(nn.Module):
+    """timm's ResNet BasicBlock: conv1 (3x3, stride) -> bn1 + ReLU -> conv2 (3x3) -> bn2 + shortcut + ReLU; the shortcut is
+    `downsample` = 1x1 conv (stride) + BatchNorm where the shape changes."""
+
+    def __init__(self, cin, cout, stride):
+        super().__init__()
+        self.conv1 = nn.Conv2d(cin, cout, 3, stride=stride, padding=1, bias=False)
+        self.bn1 = nn.BatchNorm2d(cout)
+        self.conv2 = nn.Conv2d(cout, cout, 3, padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(cout)
+        self.downsample = None
+        if stride != 1 or cin != cout:
+            self.downsample = nn.Sequential(nn.Conv2d(cin, cout, 1, stride=stride, bias=False), nn.BatchNorm2d(cout))
+        self.stride = stride
+
+    def run(self, x, emit16=True):
+        """emit16: the block output feeds a tensor-core conv next (the following block's conv1 / downsample)."""
+        y = _conv_bn(self.conv1, self.bn1, x, self.stride, emit16=True)          # feeds conv2, a 3x3 on the tensor cores
+        ds = self.downsample
+        sc = _conv_bn(ds[0], ds[1], x, self.stride, act=False) if ds is not None else x
+        return _conv_bn(self.conv2, self.bn2, y, emit16=emit16, residual=sc)
+
+
+class _Layer(_Blocks):
+    def __init__(self, cin, cout, depth, stride):
+        super().__init__()
+        for i in range(depth):
+            self.add_module(str(i), _BasicBlock(cin if i == 0 else cout, cout, stride if i == 0 else 1))
+
+
+class _ResNet(nn.Module):
+    """Parameter tree of timm's BasicBlock ResNet without its classifier (names: conv1, bn1, layer1..4.{k}.{conv1, bn1, conv2, bn2,
+    downsample.0, downsample.1}); the stem is conv1 (7x7 / 2) -> bn1 + ReLU -> 3x3 / 2 max-pool."""
+
+    def __init__(self, depths, in_chans=3):
+        super().__init__()
+        self.conv1 = nn.Conv2d(in_chans, 64, 7, stride=2, padding=3, bias=False)
+        self.bn1 = nn.BatchNorm2d(64)
+        self.feature_info = [dict(num_chs=64, reduction=2, module='act1')]
+        prev = 64
+        for i, (w, d) in enumerate(zip(RESNET_WIDTHS, depths)):
+            self.add_module('layer%d' % (i + 1), _Layer(prev, w, d, 1 if i == 0 else 2))
+            prev = w
+            self.feature_info.append(dict(num_chs=w, reduction=2 ** (i + 2), module='layer%d' % (i + 1)))
+        self.num_features = prev
+        for m in self.modules():
+            if isinstance(m, nn.Conv2d):
+                nn.init.kaiming_normal_(m.weight, mode='fan_out', nonlinearity='relu')
+        for m in self.modules():
+            if isinstance(m, _BasicBlock):
+                nn.init.zeros_(m.bn2.weight)                 # timm zero_init_last_bn
+
+    @property
+    def stages(self):
+        return self.layer1, self.layer2, self.layer3, self.layer4
+
+    def run_stem(self, x):
+        # the pooled output feeds layer1.0.conv1 (a 3x3 on the tensor cores) and is that block's identity shortcut
+        return ops.max_pool2d(_conv_bn(self.conv1, self.bn1, x, stride=2), emit16=True)
+
+
+def _family(architecture):
+    """'regnet' / 'resnet' for the trunks this package implements; raises for every other name."""
+    if architecture == 'regnety_032':
+        return 'regnet'
+    if architecture in RESNET_DEPTHS:
+        return 'resnet'
+    if architecture.startswith('resnet'):
+        raise RuntimeError('transfuser_b200 implements the BasicBlock ResNets resnet18 / resnet34 only; %r is not one of them '
+                           '(Bottleneck ResNets are not implemented)' % (architecture,))
+    if architecture.startswith('convnext'):
+        raise RuntimeError('ConvNeXt trunks are not implemented by transfuser_b200, got %r' % (architecture,))
+    raise RuntimeError('transfuser_b200 implements the regnety_032, resnet18 and resnet34 trunks only, got %r' % (architecture,))
+
+
+def make_trunk(architecture, in_chans=3):
+    """The trunk named `architecture` (the timm model name). Every trunk has run_stem(x) and its four stages in `stages`."""
+    if _family(architecture) == 'regnet':
+        return _RegNet(in_chans=in_chans)
+    return _ResNet(RESNET_DEPTHS[architecture], in_chans=in_chans)
+
+
+def check_trunk_pair(image_architecture, lidar_architecture):
+    if _family(image_architecture) != _family(lidar_architecture):
+        raise RuntimeError('a RegNet trunk cannot be combined with a ResNet trunk (%r / %r): the fusion layers are built for the image '
+                           "trunk's stage widths, which the other trunk does not have" % (image_architecture, lidar_architecture))
+
 
 class ImageCNN(nn.Module):
     """transfuser.py:369-416 (regnet branch): `features` + the alias attributes the reference's forward goes through."""
 
     def __init__(self, architecture, normalize=True, out_features=512):
         super().__init__()
-        if architecture != 'regnety_032':
-            raise RuntimeError('transfuser_b200 implements the regnety_032 trunk only (train.py:50-53 default), got %r' % (architecture,))
         self.normalize = normalize
-        f = self.features = _RegNet()
-        f.conv1, f.bn1 = f.stem.conv, f.stem.bn
-        f.layer1, f.layer2, f.layer3, f.layer4 = f.s1, f.s2, f.s3, f.s4
+        f = self.features = make_trunk(architecture)
+        if isinstance(f, _RegNet):
+            f.conv1, f.bn1 = f.stem.conv, f.stem.bn
+            f.layer1, f.layer2, f.layer3, f.layer4 = f.s1, f.s2, f.s3, f.s4
 
 
 class LidarEncoder(nn.Module):
-    """transfuser.py:431-488: same trunk, new `conv1` with `in_channels`, `stem.conv` deleted."""
+    """transfuser.py:431-488: same trunk, new `conv1` with `in_channels` (a ResNet's keeps its key position); RegNet: `stem.conv`
+    deleted."""
 
     def __init__(self, architecture, in_channels=2, out_features=512):
         super().__init__()
-        if architecture != 'regnety_032':
-            raise RuntimeError('transfuser_b200 implements the regnety_032 trunk only, got %r' % (architecture,))
-        m = self._model = _RegNet()
-        old = m.stem.conv
-        m.conv1, m.bn1 = m.stem.conv, m.stem.bn   # same registration order as the reference (transfuser.py:446-453)
-        m.layer1, m.layer2, m.layer3, m.layer4 = m.s1, m.s2, m.s3, m.s4
+        m = self._model = make_trunk(architecture)
+        regnet = isinstance(m, _RegNet)
+        if regnet:
+            m.conv1, m.bn1 = m.stem.conv, m.stem.bn   # same registration order as the reference (transfuser.py:446-453)
+            m.layer1, m.layer2, m.layer3, m.layer4 = m.s1, m.s2, m.s3, m.s4
+        old = m.conv1
         m.conv1 = nn.Conv2d(in_channels, old.out_channels, kernel_size=old.kernel_size, stride=old.stride, padding=old.padding, bias=False)
-        del m.stem.conv
+        if regnet:
+            del m.stem.conv
 
 
 class SelfAttention(nn.Module):
@@ -233,6 +344,7 @@ class TransfuserBackbone(nn.Module):
     def __init__(self, config, image_architecture='resnet34', lidar_architecture='resnet18', use_velocity=True):
         super().__init__()
         self.config = config
+        check_trunk_pair(image_architecture, lidar_architecture)
         self.image_encoder = ImageCNN(architecture=image_architecture, normalize=True, out_features=config.perception_output_features)
         if config.use_point_pillars:
             raise RuntimeError('PointPillars LiDAR encoder is out of scope (config.py:42 default False)')
@@ -247,8 +359,10 @@ class TransfuserBackbone(nn.Module):
                 embd_pdrop=config.embd_pdrop, attn_pdrop=config.attn_pdrop, resid_pdrop=config.resid_pdrop, config=config,
                 use_velocity=use_velocity))
         c_last, c_out = info[4]['num_chs'], config.perception_output_features
-        self.change_channel_conv_image = nn.Conv2d(c_last, c_out, (1, 1))
-        self.change_channel_conv_lidar = nn.Conv2d(c_last, c_out, (1, 1))
+        # parameterless when the trunk already ends at perception_output_features (transfuser.py:92-97); forward skips them then
+        conv_or_none = (lambda: nn.Conv2d(c_last, c_out, (1, 1))) if c_last != c_out else nn.Sequential
+        self.change_channel_conv_image = conv_or_none()
+        self.change_channel_conv_lidar = conv_or_none()
         channel = config.bev_features_chanels
         self.up_conv5 = nn.Conv2d(channel, channel, (1, 1))
         self.up_conv4 = nn.Conv2d(channel, channel, (1, 1))
@@ -274,11 +388,11 @@ class TransfuserBackbone(nn.Module):
         x = ops.image_prep(image) if self.image_encoder.normalize else ops.nchw_to_nhwc(image)
         l = ops.nchw_to_nhwc(lidar)
         if not self.two_streams:
-            x = ie.stem.run(x, emit16=True)
-            l = ops.batch_norm(ops.conv2d(l, le.conv1.weight, None, 2, 1), le.bn1, True, le.bn1.training, emit16=True)
+            x = ie.run_stem(x)
+            l = le.run_stem(l)
             for i in range(1, 5):
-                x = getattr(ie, 's%d' % i).run(x, last16=False)
-                l = getattr(le, 's%d' % i).run(l, last16=False)
+                x = ie.stages[i - 1].run(x, last16=False)
+                l = le.stages[i - 1].run(l, last16=False)
                 x, l = getattr(self, 'transformer%d' % i).run(x, l, velocity)
                 if taps is not None:
                     taps['img_s%d' % i], taps['lid_s%d' % i] = x, l
@@ -290,12 +404,12 @@ class TransfuserBackbone(nn.Module):
             side = ops.side_stream(image.device)
             side.wait_stream(main)
             with torch.cuda.stream(side):
-                l = ops.batch_norm(ops.conv2d(l, le.conv1.weight, None, 2, 1), le.bn1, True, le.bn1.training, emit16=True)
-            x = ie.stem.run(x, emit16=True)
+                l = le.run_stem(l)
+            x = ie.run_stem(x)
             for i in range(1, 5):
                 with torch.cuda.stream(side):
-                    l = getattr(le, 's%d' % i).run(l, last16=False)
-                x = getattr(ie, 's%d' % i).run(x, last16=False)
+                    l = le.stages[i - 1].run(l, last16=False)
+                x = ie.stages[i - 1].run(x, last16=False)
                 main.wait_stream(side)
                 ops.record_stream(l, main)
                 x, l = getattr(self, 'transformer%d' % i).run(x, l, velocity)
@@ -304,8 +418,7 @@ class TransfuserBackbone(nn.Module):
                 if i < 4:
                     side.wait_stream(main)
                     ops.record_stream(l, side)
-        x = ops.conv2d(x, self.change_channel_conv_image.weight, self.change_channel_conv_image.bias)
-        l = ops.conv2d(l, self.change_channel_conv_lidar.weight, self.change_channel_conv_lidar.bias)
+        x, l = _conv1x1_or_skip(self.change_channel_conv_image, x), _conv1x1_or_skip(self.change_channel_conv_lidar, l)
         fused = ops.add(ops.PoolHWFn.apply(x), ops.PoolHWFn.apply(l))
         f = self.config.bev_upsample_factor
         up = lambda t: ops.upsample(t, t.shape[1] * f, t.shape[2] * f, False, emit16=True)
@@ -320,30 +433,33 @@ class TransfuserBackbone(nn.Module):
         return tuple(ops.nhwc_to_nchw(f) for f in feats), ops.nhwc_to_nchw(grid), fused
 
 
+def _conv1x1_or_skip(conv, x):
+    """The channel-change / channel-reduction 1x1 conv, or x itself where the reference made it a parameterless nn.Sequential()."""
+    return ops.conv2d(x, conv.weight, conv.bias) if isinstance(conv, nn.Conv2d) else x
+
+
 class _PlainEncoder(nn.Module):
     """late_fusion.py:114-163: the timm trunk used whole (stem -> s1..s4); classifier parts replaced by empty Sequentials."""
 
     def __init__(self, architecture, attr, in_chans=3, normalize=True):
         super().__init__()
-        if architecture != 'regnety_032':
-            raise RuntimeError('transfuser_b200 implements the regnety_032 trunk only, got %r' % (architecture,))
         self.normalize = normalize
-        net = _RegNet(in_chans=in_chans)
+        net = make_trunk(architecture, in_chans=in_chans)      # late_fusion.py:158: the LiDAR trunk is built with in_chans
         net.fc, net.classifier, net.global_pool, net.head = nn.Sequential(), nn.Sequential(), nn.Sequential(), nn.Sequential()
         setattr(self, attr, net)
         object.__setattr__(self, '_net', net)
 
     def run(self, x):
         net = self._net
-        x = net.stem.run(x, emit16=True)
-        for i in range(1, 5):
-            x = getattr(net, 's%d' % i).run(x)
+        x = net.run_stem(x)
+        for stage in net.stages:
+            x = stage.run(x)
         return x
 
 
 class LateFusionBackbone(nn.Module):
     """H100-native drop-in for team_code_transfuser/late_fusion.py:5-111 (BASELINE config 5): two independent
-    RegNetY trunks, 1x1 channel reduction, global pools summed, FPN top-down on the LiDAR grid. Same parameter names."""
+    trunks, 1x1 channel reduction, global pools summed, FPN top-down on the LiDAR grid. Same parameter names."""
 
     def __init__(self, config, image_architecture='resnet34', lidar_architecture='resnet18', use_velocity=0):
         super().__init__()
@@ -353,14 +469,18 @@ class LateFusionBackbone(nn.Module):
         if use_velocity:
             raise RuntimeError('use_velocity=True is not implemented (train.py:54 default is 0)')
         in_channels = 2 * config.lidar_seq_len + (1 if config.use_target_point_image else 0)
+        check_trunk_pair(image_architecture, lidar_architecture)
         self.image_encoder = _PlainEncoder(image_architecture, 'features', 3, normalize=True)
         self.lidar_encoder = _PlainEncoder(lidar_architecture, '_model', in_channels, normalize=False)
         self.norm_after_pool_img = nn.Sequential()
         self.norm_after_pool_lidar = nn.Sequential()
         self.use_velocity = use_velocity
-        channel, c_out, c_last = config.bev_features_chanels, config.perception_output_features, REGNETY_032['widths'][-1]
-        self.reduce_channels_conv_image = nn.Conv2d(c_last, c_out, (1, 1))
-        self.reduce_channels_conv_lidar = nn.Conv2d(c_last, c_out, (1, 1))
+        channel, c_out = config.bev_features_chanels, config.perception_output_features
+        # both parameterless when the IMAGE trunk already ends at perception_output_features (late_fusion.py:45-52: "ResNet
+        # models were trained without this"); forward skips them then
+        c_img, c_lid = self.image_encoder._net.num_features, self.lidar_encoder._net.num_features
+        self.reduce_channels_conv_image = nn.Conv2d(c_img, c_out, (1, 1)) if c_img != c_out else nn.Sequential()
+        self.reduce_channels_conv_lidar = nn.Conv2d(c_lid, c_out, (1, 1)) if c_img != c_out else nn.Sequential()
         self.up_conv5 = nn.Conv2d(channel, channel, (1, 1))
         self.up_conv4 = nn.Conv2d(channel, channel, (1, 1))
         self.up_conv3 = nn.Conv2d(channel, channel, (1, 1))
@@ -387,8 +507,7 @@ class LateFusionBackbone(nn.Module):
         else:
             x = self.image_encoder.run(ops.image_prep(image))
             l = self.lidar_encoder.run(ops.nchw_to_nhwc(lidar))
-        x = ops.conv2d(x, self.reduce_channels_conv_image.weight, self.reduce_channels_conv_image.bias)
-        l = ops.conv2d(l, self.reduce_channels_conv_lidar.weight, self.reduce_channels_conv_lidar.bias)
+        x, l = _conv1x1_or_skip(self.reduce_channels_conv_image, x), _conv1x1_or_skip(self.reduce_channels_conv_lidar, l)
         fused = ops.add(ops.PoolHWFn.apply(x), ops.PoolHWFn.apply(l))
         f = self.config.bev_upsample_factor
         up = lambda t: ops.upsample(t, t.shape[1] * f, t.shape[2] * f, False, emit16=True)
@@ -409,8 +528,9 @@ class _GeoLidarEncoder(nn.Module):
 
     def __init__(self, architecture, in_channels=2):
         super().__init__()
-        if architecture != 'regnety_032':
-            raise RuntimeError('transfuser_b200 implements the regnety_032 trunk only, got %r' % (architecture,))
+        if _family(architecture) != 'regnet':
+            raise RuntimeError('the geometric_fusion and latentTF LiDAR encoders delete the trunk\'s `stem` (geometric_fusion.py:404, '
+                               'latentTF.py:416), which a ResNet does not have: the reference cannot build them with %r' % (architecture,))
         m = self._model = _RegNet()
         old = m.stem.conv
         m.conv1, m.bn1 = m.stem.conv, m.stem.bn
@@ -446,6 +566,7 @@ class GeometricFusionBackbone(nn.Module):
             raise RuntimeError('n_scale=%r is not implemented (config.py default 4)' % (config.n_scale,))
         self.use_velocity = use_velocity
         in_channels = 2 * config.lidar_seq_len + (1 if config.use_target_point_image else 0)
+        check_trunk_pair(image_architecture, lidar_architecture)
         self.image_encoder = ImageCNN(architecture=image_architecture, normalize=True)
         self.lidar_encoder = _GeoLidarEncoder(architecture=lidar_architecture, in_channels=in_channels)
         widths, hid = REGNETY_032['widths'], config.n_embd

@@ -782,9 +782,70 @@ class Subsample2Fn(Function):
         return dx
 
 
+class Conv7x7Fn(Function):
+    """The ResNet stem conv: 7x7 / stride 2 / pad 3, no bias, <= 4 input channels (csrc/resnet_stem.cu), exact fp32 in every mode.
+    Forward and weight gradient only: the trunk inputs (image, LiDAR BEV) never need a gradient."""
+
+    @staticmethod
+    def forward(ctx, x, w):
+        x = _c(x)
+        N, H, W, Cin = x.shape
+        y = torch.empty((N, (H - 1) // 2 + 1, (W - 1) // 2 + 1, w.shape[0]), dtype=torch.float32, device=x.device)
+        call('tfb_conv7x7s2_fwd', x, _c(w), y, N, H, W, Cin, w.shape[0])
+        ctx.save_for_backward(x, w)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        if ctx.needs_input_grad[0]:
+            raise RuntimeError('the 7x7 stem conv has no input gradient (csrc/resnet_stem.cu): its input must not require grad')
+        x, w = ctx.saved_tensors
+        N, H, W, Cin = x.shape
+        dw = None
+        if ctx.needs_input_grad[1]:
+            dw = _gbuf(w)
+            call('tfb_conv7x7s2_wgrad', x, _c(dy), dw, N, H, W, Cin, w.shape[0])
+        return None, dw
+
+
+class MaxPool2dFn(Function):
+    """max_pool2d(x, 3, stride 2, padding 1) with PyTorch's semantics (csrc/resnet_stem.cu): the forward keeps a one-byte argmax
+    tap per output element, the backward gathers each input element's gradient from the <= 4 windows that selected it."""
+
+    @staticmethod
+    def forward(ctx, x, emit16):
+        x = _c(x)
+        N, H, W, C = x.shape
+        y = torch.empty((N, (H - 1) // 2 + 1, (W - 1) // 2 + 1, C), dtype=torch.float32, device=x.device)
+        y16 = _emit16(y, emit16)
+        arg = torch.empty(y.shape, dtype=torch.uint8, device=x.device)
+        call('tfb_maxpool3x3s2_fwd', x, y, y16, arg, N, H, W, C)
+        ctx.save_for_backward(arg)
+        ctx.shape = (N, H, W, C)
+        return _attach16(y, y16)
+
+    @staticmethod
+    def backward(ctx, dy):
+        arg, = ctx.saved_tensors
+        N, H, W, C = ctx.shape
+        dx = torch.empty((N, H, W, C), dtype=torch.float32, device=dy.device)
+        call('tfb_maxpool3x3s2_bwd', _c(dy), arg, dx, N, H, W, C)
+        return dx, None
+
+
+def max_pool2d(x, emit16=False):
+    """3x3 / stride-2 / pad-1 max-pool of the NHWC tensor x. emit16: the output feeds a tensor-core conv next (bf16 mode: its bf16
+    copy is written in the same pass)."""
+    return MaxPool2dFn.apply(x, emit16)
+
+
 def conv2d(x, w, bias=None, stride=1, groups=1, relu=False, bn_stats=False):
     """bn_stats: a training-mode BatchNorm consumes the result next — on the tensor-core paths (bf16 mode) the producing kernel's
     epilogue then accumulates the per-channel sum / sum of squares (y._tfb_stats) and batch_norm skips its statistics pass."""
+    if w.shape[2] == 7:
+        if not (stride == 2 and groups == 1 and bias is None and not relu and w.shape[1] <= 4):
+            raise RuntimeError('7x7 convs are implemented for the ResNet stem only (stride 2, no bias / ReLU, <= 4 input channels)')
+        return Conv7x7Fn.apply(x, w)
     bn_stats = bn_stats and BN_STATS_FUSED and G.MODE == 'bf16' and bias is None and not relu
     if w.shape[2] == 1 and stride == 2 and groups == 1 and (G.MODE == 'bf16' or G.multi_term()):
         x, stride = Subsample2Fn.apply(x), 1
