@@ -20,6 +20,13 @@ class TrainConfig:
     use_point_pillars = False
     max_lidar_points = 40000
     backbone = 'transFuser'
+    # camera pre-processing and rotation augmentation of the dataset reader (config.py:11-13, 32-34)
+    scale = 1
+    img_resolution = (160, 704)
+    img_width = 320
+    augment = True
+    inv_augment_prob = 0.1
+    aug_max_rotation = 20
     # inference-side box decode (config.py:16, 39, 58-62)
     pixels_per_meter = 8.0
     bb_confidence_threshold = 0.3

@@ -10,7 +10,10 @@ inputs in HBM (csrc/input_prep.cu, csrc/bev_hist.cu):
     losses = model(batch['rgb'], batch['lidar'], target_point_image=batch['target_point_image'], ...)
 
 Host-side pieces that stay numpy, as in the reference (tiny, per sample): the pose algebra of align() (data.py:413-431) and
-the augmentation draw. JPEG/PNG decoding, label parsing and the BEV-label rotation (skimage) are not part of this module."""
+the augmentation draw. With the topdown plane and the matrix of bev_rotation_matrix, a fourth launch builds the rotated BEV label
+(csrc/bev_label.cu, skimage's rotate in load_crop_bev_npy). PNG decoding and label parsing stay on the host (dataset.py)."""
+import math
+
 import numpy as np
 import torch
 
@@ -32,6 +35,29 @@ def align_transform(ego_matrix_0, ego_matrix_1, degree=0.0):
 def crop_shift_pixels(degree, img_width, scale):
     """data.py:219: horizontal crop shift that accompanies an augmentation yaw of `degree` (truncated like int())."""
     return int(degree / 60 * img_width / scale)
+
+
+def _mat3(a, b):
+    return [[(a[i][0] * b[0][j] + a[i][1] * b[1][j]) + a[i][2] * b[2][j] for j in range(3)] for i in range(3)]
+
+
+def bev_rotation_matrix(degree, H, W):
+    """The 2x3 float64 output -> input matrix of skimage.transform.rotate(image of H x W, degree) that load_crop_bev_npy
+    (data.py:601) applies to the BEV label, as the [6] row-major input of tfb_bev_label_prep.
+
+    skimage composes translate(-c) -> rotate(rad) -> translate(c), c = (W/2 - 0.5, H/2 - 0.5), as T1 . (R . T3). This computes
+    it in scalar Python floats: rad = degree * (pi / 180) (np.deg2rad), math.cos / math.sin, and every entry of the two 3x3
+    products as ((a0*b0 + a1*b1) + a2*b2). It equals skimage's matrix on a BLAS without fused multiply-add (numpy's `@` may go
+    through an FMA dgemm, which would make the result depend on the host)."""
+    degree = float(degree)
+    cx, cy = W / 2. - 0.5, H / 2. - 0.5
+    rad = degree * (math.pi / 180)
+    t1 = [[math.cos(0.0), -math.sin(0.0), cx], [math.sin(0.0), math.cos(0.0), cy], [0.0, 0.0, 1.0]]
+    t2 = [[math.cos(rad), -math.sin(rad), 0.0], [math.sin(rad), math.cos(rad), 0.0], [0.0, 0.0, 1.0]]
+    t3 = [[math.cos(0.0), -math.sin(0.0), -cx], [math.sin(0.0), math.cos(0.0), -cy], [0.0, 0.0, 1.0]]
+    m = _mat3(t1, _mat3(t2, t3))
+    assert m[2] == [0.0, 0.0, 1.0], m[2]        # affine: the kernel's projective divide is by exactly 1
+    return np.array(m[0] + m[1], dtype=np.float64)
 
 
 class InputPipeline:
@@ -68,10 +94,12 @@ class InputPipeline:
         """raw (host or device tensors):
              rgb [B,H,W,3] uint8 (RGB), optional depth [B,H,W,3] uint8, seg [B,H,W] uint8, crop_shift [B] int32 (host values),
              points [B,N,4] float32 (padded), optional n_valid [B] int32, transforms [B,4,4] float64 (align_transform),
-             target_point [B,2] float64.
+             target_point [B,2] float64, optional bev_u8 [B,H,W] uint8 (RGB plane 2 of topdown/encoded_*.png) with bev_matrix
+             [B,6] float64 (bev_rotation_matrix of each sample's augmentation angle).
            Returns rgb [B,3,h,w] float32 0..255 (or, with normalized_nhwc, the normalised NHWC tensor the backbone consumes
            directly), lidar [B,2,256,256], target_point_image [B,1,256,256], target_point [B,2] float32, and depth [B,h,w] /
-           semantic [B,h,w] int64 when their sources are given. `out` (optional dict) supplies preallocated destinations
+           semantic [B,h,w] int64 when their sources are given, and the rotated BEV label bev [B,160,160] int64
+           (load_crop_bev_npy, csrc/bev_label.cu) when bev_u8 is given. `out` (optional dict) supplies preallocated destinations
            by the same keys, so the three launches can write straight into the static inputs of a captured training step."""
         self._require_cuda()
         res = {}
@@ -126,4 +154,20 @@ class InputPipeline:
         tpf = self._out(out, 'target_point', (B, 2), torch.float32)
         tpf.copy_(tp)
         res['target_point'] = tpf
+
+        if (raw.get('bev_u8') is None) != (raw.get('bev_matrix') is None):
+            raise ValueError('bev_u8 and bev_matrix go together')
+        if raw.get('bev_u8') is not None:
+            plane = self._dev(raw['bev_u8'], torch.uint8)
+            m = torch.as_tensor(raw['bev_matrix'])
+            if plane.dim() != 3 or plane.shape[0] != B or plane.shape[1] < 250 or plane.shape[2] < 330:
+                raise ValueError('bev_u8 must be [B, H >= 250, W >= 330] uint8, got %s' % (tuple(plane.shape),))
+            if tuple(m.shape) != (B, 6):
+                raise ValueError('bev_matrix must be [B, 6] float64 (bev_rotation_matrix), got %s' % (tuple(m.shape),))
+            if not m.is_cuda and not bool(torch.isfinite(m).all()):
+                raise ValueError('bev_matrix holds a non-finite value')
+            m = self._dev(m, torch.float64)
+            bev_out = self._out(out, 'bev', (B, 160, 160), torch.int64)
+            _lib.call('tfb_bev_label_prep', plane, m, B, plane.shape[1], plane.shape[2], bev_out)
+            res['bev'] = bev_out
         return res

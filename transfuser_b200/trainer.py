@@ -18,6 +18,9 @@ INPUT_KEYS = ('rgb', 'points', 'target_point_image', 'target_point', 'ego_vel', 
 # the GPU input pipeline (pipeline.InputPipeline, csrc/input_prep.cu) builds the model inputs inside the step — 1.6 MB instead of
 # 3.8 MB per sample over PCIe
 RAW_KEYS = ('rgb_u8', 'depth_u8', 'seg_u8', 'crop_shift', 'points', 'transforms', 'target_point64', 'ego_vel', 'ego_waypoint', 'bev', 'label')
+# raw_inputs='dataset': the batches of dataset.CarlaRawDataset / dataset.collate — the raw inputs with the sweep's point count and, in
+# place of the finished BEV label, the topdown plane and the augmentation's rotation matrix (rotated inside the step, csrc/bev_label.cu)
+DATASET_KEYS = tuple(k for k in RAW_KEYS if k != 'bev') + ('n_valid', 'bev_u8', 'bev_matrix')
 
 
 class Trainer:
@@ -26,7 +29,9 @@ class Trainer:
         self.cfg, self.device = cfg, device
         # the geometric-fusion backbone consumes two more inputs per sample (train.py:279-288)
         self.raw_inputs = raw_inputs
-        self.input_keys = (RAW_KEYS if raw_inputs else INPUT_KEYS) + (('bev_points', 'cam_points') if backbone == 'geometric_fusion' else ())
+        if raw_inputs not in (False, True, 'dataset'):
+            raise ValueError("raw_inputs must be False, True or 'dataset'")
+        self.input_keys = (DATASET_KEYS if raw_inputs == 'dataset' else RAW_KEYS if raw_inputs else INPUT_KEYS) + (('bev_points', 'cam_points') if backbone == 'geometric_fusion' else ())
         if raw_inputs:
             from .pipeline import InputPipeline
             self.pipe = InputPipeline(cfg, device)
@@ -83,10 +88,13 @@ class Trainer:
     def _step(self, d):
         if self.raw_inputs:
             # crop + CHW / normalise, depth decode, class LUT, align + BEV histogram, target-point map: three launches on the raw batch
-            p = self.pipe.prepare(dict(rgb=d['rgb_u8'], depth=d['depth_u8'], seg=d['seg_u8'], crop_shift=d['crop_shift'], points=d['points'],
-                                       transforms=d['transforms'], target_point=d['target_point64']), normalized_nhwc=True)
+            raw = dict(rgb=d['rgb_u8'], depth=d['depth_u8'], seg=d['seg_u8'], crop_shift=d['crop_shift'], points=d['points'],
+                       transforms=d['transforms'], target_point=d['target_point64'])
+            if self.raw_inputs == 'dataset':
+                raw.update(n_valid=d['n_valid'], bev_u8=d['bev_u8'], bev_matrix=d['bev_matrix'])   # + the BEV-label rotation
+            p = self.pipe.prepare(raw, normalized_nhwc=True)
             d = dict(d, rgb=p['rgb'], depth=p['depth'], semantic=p['semantic'], target_point=p['target_point'],
-                     target_point_image=p['target_point_image'])
+                     target_point_image=p['target_point_image'], bev=p.get('bev', d.get('bev')))
             lidar = p['lidar']
         else:
             lidar = bev.lidar_to_histogram_features_batched(d['points'])
