@@ -56,7 +56,7 @@ __global__ void __launch_bounds__(256) ce_fwd_kernel(const float* __restrict__ l
     for (int c = 0; c < kMaxC; ++c) if (c == t) lt = v[c];
     float w = class_w ? class_w[t] : 1.f;
     if (pos_w) w *= pos_w[m % HW];
-    ls = fmaf(w, (logf(se) + mx - lt), ls);
+    ls = fmaf(w, logf(se) - (lt - mx), ls);   // as log_softmax: adding mx first would drop the low bits of log(se)
     ws += w;
   }
   block_partial(part, 2, 0, ls, red);
@@ -277,7 +277,7 @@ __global__ void __launch_bounds__(256) centernet_loss_kernel(const float* __rest
 #pragma unroll
       for (int c = 0; c < 12; ++c) se += expf(P[5 + c] - mx);
       const int t = (int)T[8 * HW];
-      if (MODE == 0) s[3] += Wsum * (logf(se) + mx - P[5 + t]);
+      if (MODE == 0) s[3] += Wsum * (logf(se) - (P[5 + t] - mx));   // x_t - mx first, as in ce_fwd_kernel
       else {
 #pragma unroll
         for (int c = 0; c < 12; ++c) D[5 + c] = coef[3] * Wsum * (expf(P[5 + c] - mx) / se - (c == t ? 1.f : 0.f));
@@ -288,7 +288,7 @@ __global__ void __launch_bounds__(256) centernet_loss_kernel(const float* __rest
       const float mx = fmaxf(a, bq);
       const float ea = expf(a - mx), eb = expf(bq - mx), se = ea + eb;
       const int t = (int)T[9 * HW];
-      if (MODE == 0) s[6] += Wsum * (logf(se) + mx - (t == 0 ? a : bq));
+      if (MODE == 0) s[6] += Wsum * (logf(se) - ((t == 0 ? a : bq) - mx));
       else {
         D[19] = coef[6] * Wsum * (ea / se - (t == 0 ? 1.f : 0.f));
         D[20] = coef[6] * Wsum * (eb / se - (t == 1 ? 1.f : 0.f));
