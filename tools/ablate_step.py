@@ -22,7 +22,7 @@ DEFAULT_SETS = [
     'tfb_gemm_bf16_tc+tfb_gemm_bf16_tc_stats+tfb_gemm_bf16_tc_out16', 'tfb_conv3x3_tc+tfb_conv3x3_tc_strided',
     'tfb_layernorm_bwd+tfb_layernorm_fwd+tfb_dropout+tfb_add_dropout_ln_fwd+tfb_add_dropout_ln_bwd+tfb_attn_fwd_tc+tfb_attn_bwd_tc',
     'tfb_grad_prep+tfb_cast_bf16+tfb_dilate2+tfb_subsample2+tfb_colsum',
-    'tfb_im2col3x3_bf16+tfb_gemm_bf16_tc_wgrad_batched', 'tfb_upsample_bilinear_bwd+tfb_upsample_bilinear_fwd+tfb_gpt_up_add_fwd+tfb_gpt_up_add_bwd',
+    'tfb_im2col3x3_bf16+tfb_gemm_bf16_tc_wgrad_batched', 'tfb_conv3x3_tc_wgrad', 'tfb_upsample_bilinear_bwd+tfb_upsample_bilinear_fwd+tfb_gpt_up_add_fwd+tfb_gpt_up_add_bwd',
 ]
 
 

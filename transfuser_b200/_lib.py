@@ -112,7 +112,7 @@ class Profiler:
     FAMILY = {'tfb_gemm_bf16_tc': 'gemm_tc_kernel', 'tfb_gemm_bf16_tc_stats': 'gemm_tc_kernel', 'tfb_gemm_bf16_tc_out16': 'gemm_tc_kernel',
               'tfb_gemm_bf16_tc_wgrad_batched': 'gemm_tc_kernel', 'tfb_conv3x3_tc': 'conv3x3_tc_kernel', 'tfb_conv3x3_tc_strided': 'conv3x3_tc_kernel',
               'tfb_bn_fwd': 'bn_fwd (colreduce4 + bn_apply)', 'tfb_bn_fwd_stats': 'bn_apply_stats_kernel', 'tfb_attn_fwd_tc': 'attn_tc_kernel',
-              'tfb_attn_bwd_tc': 'attn_tc_kernel'}
+              'tfb_attn_bwd_tc': 'attn_tc_kernel', 'tfb_conv3x3_tc_wgrad': 'gemm_tc_kernel'}
 
     def __init__(self, keep_calls=False):
         self.records = []
@@ -150,6 +150,8 @@ class Profiler:
         if name.startswith('tfb_conv2d'):
             i0 = 3 if name.endswith('dgrad') else 4
             return '%s N%d H%d W%d Cin%d Cout%d k%d s%d g%d' % ((name,) + tuple(a[i0:i0 + 8]))
+        if name == 'tfb_conv3x3_tc_wgrad':
+            return '%s N%d H%d W%d Cin%d Cout%d ldg%d g%d s%d' % ((name,) + tuple(a[4:12]))
         return name
 
     @staticmethod
@@ -186,6 +188,11 @@ class Profiler:
             N, H, W, Cin, Cout, ks, stride, groups = a[i0:i0 + 8]
             Ho, Wo = (H + 2 * (ks // 2) - ks) // stride + 1, (W + 2 * (ks // 2) - ks) // stride + 1
             return 2.0 * N * Ho * Wo * Cout * (Cin // groups) * ks * ks, 4.0 * (N * H * W * Cin + N * Ho * Wo * Cout)
+        if name == 'tfb_conv3x3_tc_wgrad':
+            # bf16 x and dy read once, fp32 dW written once
+            N, H, W, Cin, Cout, ldg, groups, st = a[4:12]
+            Ho, Wo = (H - 1) // st + 1, (W - 1) // st + 1
+            return 2.0 * N * Ho * Wo * Cout * (Cin // groups) * 9, 2.0 * (N * H * W * Cin + N * Ho * Wo * ldg) + 4.0 * Cout * (Cin // groups) * 9
         b = sum(t.numel() * t.element_size() for t in a if isinstance(t, torch.Tensor))
         return 0.0, float(b)
 

@@ -11,6 +11,7 @@
 // between TMA and the MMAs.
 // Replaces cuBLAS/cuDNN behind nn.Linear and 1x1 nn.Conv2d (transfuser.py:510-527,538-543; timm RegNet 1x1 convs).
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -47,13 +48,23 @@ constexpr int kSmemMax = 232448 - 256;                        // 227 KB opt-in l
 constexpr int kSmemFixed = 256 + 8 * kStageFloats * 4 + 1024; // barriers + epilogue staging + alignment slack
 constexpr int64_t kPostFoldBytes = 256 * 1024;                // split-K partials one CTA folds at most (see launch_bn)
 
-template <typename T, bool A_MN, bool B_MN, int BN>
-__global__ void __launch_bounds__(kThreads, 1)
+// The B operand of the 3x3-conv weight gradient gathered from the bf16 activation instead of read from an im2col matrix (GATHER).
+// B[k][c] = x[n, ho*stride + kh - 1, wo*stride + kw - 1, g*Cig + ci] (0 outside the image), k = (n*Ho + ho)*Wo + wo, for the
+// column c = g*9*Cig + (kh*3 + kw)*Cig + ci: tap-major inside a group, so 8 consecutive columns are one 16-byte run of one pixel.
+struct ConvGather {
+  const __nv_bfloat16* x;
+  int H, W, Cin, Cig, Ho, Wo, stride, K, ncols;
+};
+
+constexpr int kGatherThreads = kThreads + 96;                 // GATHER: warps 8-11 produce (168 registers x 384 threads fit)
+
+template <typename T, bool A_MN, bool B_MN, int BN, bool GATHER = false>
+__global__ void __launch_bounds__(GATHER ? kGatherThreads : kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, float* __restrict__ Cbase,
                int64_t ldc, int M, int N, int num_kb, int kb_per_split, const float* __restrict__ bias, float alpha, float beta,
                int relu, int atomic_out, int splits, int a_step, int b_step, int64_t c_bstride, int tiles_m, int tiles_n,
                int total_tiles, int STAGES, double* __restrict__ stats, __nv_bfloat16* __restrict__ C16, float* __restrict__ ws,
-               unsigned int* __restrict__ ws_cnt) {
+               unsigned int* __restrict__ ws_cnt, const ConvGather cg) {
   // PERSISTENT: gridDim.x CTAs (<= one per SM) walk the tile list t = blockIdx.x, += gridDim.x. A tile is (m-tile, n-tile, z),
   // z = batch * splits + split; m fastest so that concurrently running CTAs share the same B (weight) tile in L2.
   // Consumer warpgroup g (warps 4g..4g+3) owns rows [64g, 64g + 64) of the 128 x BN tile as a wgmma register accumulator;
@@ -73,7 +84,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tma_a);
     tc::tma_prefetch_desc(&tma_b);
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 8); }   // 8 consumer warps
+    // GATHER: every producer thread arrives once its cp.async copies of the B tile have landed
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], GATHER ? 128 : 1); tc::mbar_init(&empty_bar[s], 8); }   // 8 consumer warps
     tc::mbar_fence_init();
   }
   __syncthreads();
@@ -89,7 +101,52 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     nkb = min(num_kb, kb_begin + kb_per_split) - kb_begin;   // >= 1 by construction
   };
 
-  if (warp == 8) {
+  if (GATHER && warp >= 8) {
+    // ===== producers (warps 8-11): A by TMA (thread 256), B gathered with 16-byte cp.async, two threads per pixel row =====
+    static_assert(!GATHER || (sizeof(T) == 2 && A_MN && B_MN), "the gathered B is the bf16 wgrad form");
+    int s = 0, ph = 0;
+    constexpr int nb_chunks = (BN + E::kPerRow - 1) / E::kPerRow;
+    const int hw = cg.Ho * cg.Wo, gcols = 9 * cg.Cig;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+      int m0, n0, bz, sz, kb_begin, nkb;
+      decode(t, m0, n0, bz, sz, kb_begin, nkb);
+      const int am0 = m0 + bz * a_step, bn0 = n0 + bz * b_step;
+      for (int i = 0; i < nkb; ++i) {
+        tc::mbar_wait(&empty_bar[s], ph ^ 1);
+        uint8_t* sa = smem + s * stage_bytes;
+        uint8_t* sb = sa + kABytes;
+        const int k0 = (kb_begin + i) * BK;
+        const int pt = threadIdx.x - 256, r = pt >> 1, half = pt & 1;
+        if (pt == 0) {
+          tc::mbar_expect_tx_only(&full_bar[s], kABytes);
+#pragma unroll
+          for (int j = 0; j < BM / E::kPerRow; ++j) tc::tma_load_2d(&tma_a, &full_bar[s], sa + j * BK * 128, am0 + j * E::kPerRow, k0);
+        }
+        {
+          const int k = k0 + r;
+          const bool krow = k < cg.K;
+          const int n = krow ? k / hw : 0, p = k - n * hw, ho = p / cg.Wo, wo = p - ho * cg.Wo;
+          const int c0 = bn0 + 8 * half;
+          int g = c0 / gcols, tap = (c0 - g * gcols) / cg.Cig, ci = c0 - g * gcols - tap * cg.Cig;
+#pragma unroll
+          for (int q = half; q < nb_chunks * 8; q += 2) {   // 16-byte unit q: columns bn0 + 8q ... + 7
+            const int hi = ho * cg.stride + tap / 3 - 1, wi = wo * cg.stride + tap % 3 - 1;
+            const bool in = krow && bn0 + 8 * q < cg.ncols && hi >= 0 && hi < cg.H && wi >= 0 && wi < cg.W;
+            const __nv_bfloat16* src = in ? cg.x + (((int64_t)n * cg.H + hi) * cg.W + wi) * cg.Cin + g * cg.Cig + ci : cg.x;
+            // the 128B-swizzled MN-major layout TMA would write: chunk q / 8, row r, 16-byte unit (q % 8) ^ (r % 8); zeros outside
+            tc::cp_async16(tc::smem_u32(sb + (q >> 3) * BK * 128 + r * 128 + (((q & 7) ^ (r & 7)) << 4)), src, in ? 16u : 0u);
+#pragma unroll
+            for (int step = 0; step < 2; ++step) {          // to unit q + 2
+              ci += 8;
+              if (ci == cg.Cig) { ci = 0; if (++tap == 9) { tap = 0; ++g; } }
+            }
+          }
+        }
+        tc::cp_async_mbar_arrive(&full_bar[s]);
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+    }
+  } else if (warp == 8) {
     // ===== TMA producer =====
     if (lane == 0) {
       int s = 0, ph = 0;
@@ -135,6 +192,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       int prev = 0;
       for (int i = 0; i < nkb; ++i) {
         tc::mbar_wait(&full_bar[s], ph);
+        if (GATHER) tc::fence_async_smem();      // the cp.async writes of B -> visible to wgmma (async proxy)
         const uint32_t base = tc::smem_u32(smem + s * stage_bytes);
         // this warpgroup's 64 rows: K-major A: 64 rows of 128 B further; MN-major A: the second 64-element M chunk
         const uint32_t sa = base + (A_MN ? wg * BK * 128 : wg * 64 * 128), sb = base + kABytes;
@@ -288,7 +346,7 @@ bool make_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols,
 template <typename T, bool A_MN, bool B_MN, int BN>
 int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
               int relu, float alpha, float beta, int splits, cudaStream_t stream, int nbatch = 1, int a_step = 0, int b_step = 0,
-              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr) {
+              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr, const ConvGather* gather = nullptr) {
   using E = Elem<T>;
   if (C16) {     // bf16 output: coalesced epilogue path only
     TFB_REQUIRE(splits <= 1 && beta == 0.f && (ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(C16) & 7) == 0);
@@ -309,8 +367,9 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
   if (!A_MN) ok = make_map_2d<T>(&ma, A, Mext, K, lda, BK, BM);              // A[m][k]
   else       ok = make_map_2d<T>(&ma, A, K, Mext, lda, E::kPerRow, BK);      // A[k][m]
   if (!ok) { tfb_set_last_error("cuTensorMapEncodeTiled(A) failed"); return TFB_ERR_DRIVER; }
-  if (!B_MN) ok = make_map_2d<T>(&mb, B, Next, K, ldb, BK, BN);              // B[n][k]
-  else       ok = make_map_2d<T>(&mb, B, K, Next, ldb, E::kPerRow, BK);      // B[k][n]
+  if (gather)     memset(&mb, 0, sizeof(mb));                                // B is gathered, not loaded
+  else if (!B_MN) ok = make_map_2d<T>(&mb, B, Next, K, ldb, BK, BN);         // B[n][k]
+  else            ok = make_map_2d<T>(&mb, B, K, Next, ldb, E::kPerRow, BK); // B[k][n]
   if (!ok) { tfb_set_last_error("cuTensorMapEncodeTiled(B) failed"); return TFB_ERR_DRIVER; }
   const int num_kb = (K + BK - 1) / BK;
   if (splits < 1) splits = 1;
@@ -326,13 +385,17 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
     if (beta != 0.f && beta != 1.f) { tfb_set_last_error("split-K needs beta in {0,1}"); return TFB_ERR_ARG; }
   }
   auto kern = gemm_tc_kernel<T, A_MN, B_MN, BN>;
-  static bool attr_done = false;
-  if (!attr_done) {
+  if constexpr (sizeof(T) == 2 && A_MN && B_MN) {
+    if (gather) kern = gemm_tc_kernel<T, A_MN, B_MN, BN, true>;
+  }
+  if (gather && kern == gemm_tc_kernel<T, A_MN, B_MN, BN>) { tfb_set_last_error("gathered B: bf16 wgrad form only"); return TFB_ERR_UNSUPPORTED; }
+  static bool attr_done[2] = {false, false};
+  if (!attr_done[gather ? 1 : 0]) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) != cudaSuccess) {
       tfb_set_last_error("cudaFuncSetAttribute(smem) failed");
       return TFB_ERR_DRIVER;
     }
-    attr_done = true;
+    attr_done[gather ? 1 : 0] = true;
   }
   const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
   const int64_t total = (int64_t)tiles_m * tiles_n * splits * nbatch;
@@ -352,9 +415,9 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
     const int rc = tfb_scratch(ws, (size_t)grid * 2 * N, (size_t)tiles_n, stream);
     if (rc != TFB_OK) return rc;
   }
-  kern<<<grid, kThreads, smem_total, stream>>>(ma, mb, C, ldc, M, N, num_kb, kb_per_split, bias, alpha, beta, relu, atomic_out, splits,
+  kern<<<grid, gather ? kGatherThreads : kThreads, smem_total, stream>>>(ma, mb, C, ldc, M, N, num_kb, kb_per_split, bias, alpha, beta, relu, atomic_out, splits,
                                                a_step, b_step, c_bstride, tiles_m, tiles_n, (int)total, stages, stats, C16, ws.f,
-                                               post_fold ? nullptr : ws.cnt);
+                                               post_fold ? nullptr : ws.cnt, gather ? *gather : ConvGather{});
   TFB_CHECK_LAUNCH();
   if (post_fold) {
     const int64_t n_out = (int64_t)M * N, groups = n_out % 4 == 0 ? n_out / 4 : n_out;
@@ -368,9 +431,9 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
 template <typename T, bool A_MN, bool B_MN>
 int launch_tc(int BN, int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
               int relu, float alpha, float beta, int splits, cudaStream_t stream, int nbatch = 1, int a_step = 0, int b_step = 0,
-              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr) {
+              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr, const ConvGather* gather = nullptr) {
 #define TFB_BN(bn_) case bn_: return launch_bn<T, A_MN, B_MN, bn_>(M, N, K, A, lda, B, ldb, C, ldc, bias, relu, alpha, beta, splits, stream, \
-                                                                  nbatch, a_step, b_step, c_bstride, stats, C16)
+                                                                  nbatch, a_step, b_step, c_bstride, stats, C16, gather)
   if constexpr (B_MN) {
     switch (BN) { TFB_BN(64); TFB_BN(128); TFB_BN(192); }
   } else {
@@ -459,20 +522,65 @@ int gemm_tc_any(int transA, int transB, int M, int N, int K, const T* A, int64_t
 // Batched split-K product for grouped-conv wgrad: for b < nbatch,
 //   C_b[M,N] (fp32, at C + b*c_bstride, row stride ldc) = A[:, b*a_step : +M]^T (bf16 [K, lda]) * B[:, b*b_step : +N] (bf16 [K, ldb])
 // i.e. the transA=1 / transB=0 case of tfb_gemm_bf16_tc with per-batch column windows of the same two matrices.
+namespace {
+// The batched wgrad product (tile width, split-K, fold) with B from memory or, given `gather`, gathered from the conv input.
+int wgrad_batched(int M, int N, int K, const void* A, int64_t lda, int a_step, const void* B, int64_t ldb, int b_step, float* C, int64_t ldc,
+                  int64_t c_bstride, int nbatch, int splits, cudaStream_t stream, const ConvGather* gather) {
+  using T = __nv_bfloat16;
+  const int num_kb = (K + 63) / 64;
+  if (splits <= 0) {                                                                  // auto split-K
+    const int bn = pick_bn(M, N, nbatch, 64, num_kb, true, &splits);
+    return launch_tc<T, true, true>(bn, M, N, K, (const T*)A, lda, (const T*)B, ldb, C, ldc, nullptr, 0, 1.f, 0.f, splits, stream, nbatch, a_step, b_step, c_bstride,
+                                    nullptr, nullptr, gather);
+  }
+  const int zs = (splits < 1 ? 1 : (splits > num_kb ? num_kb : splits)) * nbatch;
+  return launch_tc<T, true, true>(pick_bn(M, N, zs, 64), M, N, K, (const T*)A, lda, (const T*)B, ldb, C, ldc, nullptr, 0, 1.f, 0.f, splits, stream, nbatch, a_step, b_step,
+                                  c_bstride, nullptr, nullptr, gather);
+}
+
+// dw[co][ci][tap] = work[co][tap][ci] (the gathered product's columns are tap-major), co < Cout
+__global__ void wgrad_untap_kernel(const float* __restrict__ work, float* __restrict__ dw, int64_t n, int Cig) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t co = i / (9 * Cig);
+    const int r = (int)(i - co * 9 * Cig), ci = r / 9, tap = r - ci * 9;
+    dw[i] = work[co * 9 * Cig + tap * Cig + ci];
+  }
+}
+}  // namespace
+
 TFB_API int tfb_gemm_bf16_tc_wgrad_batched(int M, int N, int K, const void* A, int64_t lda, int a_step, const void* B, int64_t ldb,
                                            int b_step, float* C, int64_t ldc, int64_t c_bstride, int nbatch, int splits,
                                            cudaStream_t stream) {
   TFB_REQUIRE(M > 0 && N > 0 && K > 0 && A && B && C && nbatch >= 1);
   TFB_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0);
   TFB_REQUIRE(lda % 8 == 0 && ldb % 8 == 0 && a_step % 8 == 0 && b_step % 8 == 0);
-  using T = __nv_bfloat16;
-  const int num_kb = (K + 63) / 64;
-  if (splits <= 0) {                                                                  // auto split-K
-    const int bn = pick_bn(M, N, nbatch, 64, num_kb, true, &splits);
-    return launch_tc<T, true, true>(bn, M, N, K, (const T*)A, lda, (const T*)B, ldb, C, ldc, nullptr, 0, 1.f, 0.f, splits, stream, nbatch, a_step, b_step, c_bstride);
-  }
-  const int zs = (splits < 1 ? 1 : (splits > num_kb ? num_kb : splits)) * nbatch;
-  return launch_tc<T, true, true>(pick_bn(M, N, zs, 64), M, N, K, (const T*)A, lda, (const T*)B, ldb, C, ldc, nullptr, 0, 1.f, 0.f, splits, stream, nbatch, a_step, b_step, c_bstride);
+  return wgrad_batched(M, N, K, A, lda, a_step, B, ldb, b_step, C, ldc, c_bstride, nbatch, splits, stream, nullptr);
+}
+
+// Weight gradient of the 3x3 conv (pad 1, stride 1 or 2, groups) y = conv(x) without an im2col matrix: the same product, tiles, split-K
+// and fold as tfb_im2col3x3_bf16 + tfb_gemm_bf16_tc_wgrad_batched (so the same bits when x16 is the round-to-nearest bf16 copy of the
+// im2col kernel's fp32 input), with the producer gathering each B tile from x16[N,H,W,Cin]. dy16: bf16 [N,Ho,Wo,ldg] (ldg >= Cout,
+// dense; == Cout, grouped).
+// work: rows * 9 * Cin/groups floats (rows = max(Cout, ldg) dense, Cout grouped), the product in [row][tap][ci] order; dw (overwritten):
+// [Cout][Cin/groups][3][3]. splits as for tfb_gemm_bf16_tc_wgrad_batched (<= 0: chosen from the shape and the grid cap).
+TFB_API int tfb_conv3x3_tc_wgrad(const void* x16, const void* dy16, float* dw, float* work, int N, int H, int W, int Cin, int Cout, int ldg,
+                                 int groups, int stride, int splits, cudaStream_t stream) {
+  TFB_REQUIRE(x16 && dy16 && dw && work && N > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && groups >= 1 && (stride == 1 || stride == 2));
+  TFB_REQUIRE(Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % 8 == 0 && ldg % 8 == 0);
+  TFB_REQUIRE(groups == 1 ? ldg >= Cout : ((Cout / groups) % 8 == 0 && ldg == Cout));
+  TFB_REQUIRE((reinterpret_cast<uintptr_t>(x16) & 15) == 0 && (reinterpret_cast<uintptr_t>(dy16) & 15) == 0);
+  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1, Cig = Cin / groups, Cog = Cout / groups;
+  const int64_t K = (int64_t)N * Ho * Wo;
+  TFB_REQUIRE(K <= 0x7fffffff);
+  const ConvGather cg{(const __nv_bfloat16*)x16, H, W, Cin, Cig, Ho, Wo, stride, (int)K, 9 * Cin};
+  const int rows = groups > 1 ? Cog : (ldg > Cout ? ldg : Cout);
+  const int rc = wgrad_batched(rows, 9 * Cig, (int)K, dy16, ldg, groups > 1 ? Cog : 0, nullptr, 9 * Cin, groups > 1 ? 9 * Cig : 0, work, 9 * Cig,
+                               (int64_t)Cog * 9 * Cig, groups, splits, stream, &cg);
+  if (rc != TFB_OK) return rc;
+  const int64_t n = (int64_t)Cout * Cig * 9;
+  wgrad_untap_kernel<<<tfb_grid(n, 256), 256, 0, stream>>>(work, dw, n, Cig);
+  TFB_CHECK_LAUNCH();
+  return TFB_OK;
 }
 
 // TF32 operands straight from fp32 storage (wgmma .tf32). Only the K-major x K-major case (y = x W^T) exists: wgmma reads

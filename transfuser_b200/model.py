@@ -189,8 +189,13 @@ class LidarCenterNet(nn.Module):
         self.i += 1
         return pred_wp, rotated_bboxes
 
-    def forward(self, rgb, lidar_bev, ego_waypoint, target_point, target_point_image, ego_vel, bev, label, depth, semantic,
-                num_points=None, save_path=None, bev_points=None, cam_points=None):
+    def forward(self, *args, **kwargs):
+        # every 3x3 conv of the training step takes the implicit-GEMM weight gradient (bf16 mode, tensor-core shapes)
+        with ops.implicit_wgrad():
+            return self._forward(*args, **kwargs)
+
+    def _forward(self, rgb, lidar_bev, ego_waypoint, target_point, target_point_image, ego_vel, bev, label, depth, semantic,
+                 num_points=None, save_path=None, bev_points=None, cam_points=None):
         cfg = self.config
         loss = {}
         if self.use_target_point_image:

@@ -3,6 +3,7 @@ hand-written sm_90a kernel launch; torch supplies device memory, the current str
 
 Activations are NHWC fp32 ([N, H, W, C], contiguous); parameters keep the reference's PyTorch layouts so that the
 reference's state_dicts load unchanged (SURVEY.md §8b)."""
+import contextlib
 import os
 import weakref
 
@@ -108,6 +109,21 @@ DECODER_STREAMS = os.environ.get('TFB_DECODER_STREAMS', '0') == '1'   # segmenta
 BN_SE_FUSED = os.environ.get('TFB_BN_SE_FUSED', '1') == '1'     # Bottleneck conv2.bn + squeeze-excite as one autograd node (SE gradient folded into BatchNorm backward)
 ADD_LN_FUSED = os.environ.get('TFB_ADD_LN_FUSED', '1') == '1'   # GPT: residual add + dropout + the next LayerNorm in one launch
 ATTN_FUSED = os.environ.get('TFB_ATTN_FUSED', '1') == '1'       # bf16 mode: fused tensor-core attention (csrc/attn_tc.cu), no T x T tensor in HBM
+# bf16 mode: the weight gradients of the 3x3 convs made inside implicit_wgrad() (the model's forward) without the bf16 im2col
+# matrix: the wgrad GEMM gathers its tiles from the activation (tfb_conv3x3_tc_wgrad)
+IMPLICIT_WGRAD = os.environ.get('TFB_IMPLICIT_WGRAD', '1') == '1'
+_IMPLICIT_SCOPE = [0]
+
+
+@contextlib.contextmanager
+def implicit_wgrad():
+    """The 3x3 convs conv2d makes inside this context take the im2col-free weight gradient (tfb_conv3x3_tc_wgrad) when their
+    backward runs on the tensor cores; outside it they keep im2col + the batched wgrad GEMM (the same bits)."""
+    _IMPLICIT_SCOPE[0] += 1
+    try:
+        yield
+    finally:
+        _IMPLICIT_SCOPE[0] -= 1
 
 
 def _emit16(x, want):
@@ -456,7 +472,7 @@ class Conv2dFn(Function):
     """NHWC conv, k in {1,3}, pad k//2, stride {1,2}, groups. 1x1/stride-1/groups-1 goes to LinearFn instead."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, stride, groups, relu, want_stats=False):
+    def forward(ctx, x, w, bias, stride, groups, relu, want_stats=False, implicit_wgrad=False):
         x = _c(x)
         N, H, W, Cin = x.shape
         Cout, ks = w.shape[0], w.shape[2]
@@ -475,6 +491,7 @@ class Conv2dFn(Function):
             call('tfb_conv2d_fwd', x, w, bias, y, N, H, W, Cin, Cout, ks, stride, groups, int(relu))
         ctx.save_for_backward(x, w, y if relu else None, bias)
         ctx.cfg = (N, H, W, Cin, Cout, ks, stride, groups, relu, bias is not None)
+        ctx.implicit_wgrad = implicit_wgrad
         return y
 
     @staticmethod
@@ -495,7 +512,7 @@ class Conv2dFn(Function):
                 dw = _gbuf(w)
                 G.gemm_x3(G.split_bf16(g.view(-1, Cout)), _im2col_x3(x), dw.view(Cout, Cin * 9), trans_a=True)
                 db = _colsum(g.view(-1, Cout), _gbuf(bias_p)) if has_bias else None
-            return dx, dw, db, None, None, None, None
+            return dx, dw, db, None, None, None, None, None
         if ctx.needs_input_grad[0]:
             plan = _conv_tc_plan(Cout, Cin, groups) if (G.MODE == 'bf16' and ks == 3 and stride == 2) else None
             if plan is not None:
@@ -510,14 +527,14 @@ class Conv2dFn(Function):
         if ctx.needs_input_grad[1]:
             if G.MODE == 'bf16' and ks == 3 and Cout % 8 == 0 and _conv_wgrad_tc_ok(x.shape, Cout, groups, stride):
                 g16 = _take16(dy) if not relu else None       # (the 3-channel stems stay on the direct kernel: no cast for them)
-                dw = _conv_wgrad_tc(x, g16 if g16 is not None else G.to_bf16(g), w, groups, stride)
+                dw = _conv_wgrad_tc(x, g16 if g16 is not None else G.to_bf16(g), w, groups, stride, ctx.implicit_wgrad)
                 if dw is not None and has_bias:
                     db = _colsum(g.view(-1, Cout), _gbuf(bias_p))
             if dw is None:
                 dw = _gbuf(w)
                 db = _gbuf(bias_p) if has_bias else None
                 call('tfb_conv2d_wgrad', x, g, dw, db, N, H, W, Cin, Cout, ks, stride, groups)
-        return dx, dw, db, None, None, None, None
+        return dx, dw, db, None, None, None, None, None
 
 
 def _conv_x3_ok(x_shape, Cout, ks, stride, groups):
@@ -663,10 +680,12 @@ def _conv_wgrad_tc_ok(x_shape, Cout, groups, stride):
     return N * ((H - 1) // stride + 1) * ((W - 1) // stride + 1) >= 512
 
 
-def _conv_wgrad_tc(x, g16, w, groups, stride):
-    """dW of a 3x3 conv on the tensor cores: im2col(x) in bf16 with (channel, tap) column order, then one split-K GEMM per channel
-    group (dW_g[Cog, Cig*9] = dy_g^T col_g, batched over groups in a single launch) that writes PyTorch's [co][ci][kh][kw] layout
-    directly into the gradient buffer. Returns None when the shape does not fit (channel windows must be 16-byte aligned)."""
+def _conv_wgrad_tc(x, g16, w, groups, stride, implicit=False):
+    """dW of a 3x3 conv on the tensor cores: one split-K GEMM per channel group (dW_g[Cog, Cig*9] = dy_g^T col_g, batched over groups
+    in a single launch) over the bf16 im2col matrix col of x, written in PyTorch's [co][ci][kh][kw] layout into the gradient buffer.
+    implicit: the GEMM's producer gathers each tile of col from the bf16 copy of x (tfb_conv3x3_tc_wgrad) instead of reading a matrix that
+    tfb_im2col3x3_bf16 wrote; same tiles, split and fold, so the same bits. Returns None when the shape does not fit (channel
+    windows must be 16-byte aligned)."""
     N, H, W, Cin = x.shape
     Cout = w.shape[0]
     Cig, Cog = Cin // groups, Cout // groups
@@ -674,11 +693,19 @@ def _conv_wgrad_tc(x, g16, w, groups, stride):
         return None
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     M = N * Ho * Wo
-    # the seven CenterNet heads and the BEV head all convolve the same p2 map: its im2col matrix is built once per backward
-    key = (x.data_ptr(), tuple(x.shape), stride, groups)
     ldg = g16.shape[-1]                      # > Cout when dy was zero-padded to 8 channels (the 7- / 1-channel decoder outputs)
     rows = max(Cout, ldg) if groups == 1 else Cout
+    ntiles = groups * ((9 * Cig + 127) // 128)
+    splits = 0 if WGRAD_AUTO_SPLIT else max(1, min(128, (2 * 132 + ntiles - 1) // ntiles, M // 256))
     dw = _gbuf(w)
+    if implicit and IMPLICIT_WGRAD and 'tfb_conv3x3_tc_wgrad' in _lib.lib().fns:
+        x16 = _as16(x)                       # (the producers' bf16 copies round to nearest, as the im2col kernel does)
+        with _OnWgradStream(x.device, x16, g16, dw):
+            work = torch.empty(rows * 9 * Cig, dtype=torch.float32, device=x.device)
+            call('tfb_conv3x3_tc_wgrad', x16, g16, dw, work, N, H, W, Cin, Cout, ldg, groups, stride, splits)
+        return dw
+    # the seven CenterNet heads and the BEV head all convolve the same p2 map: its im2col matrix is built once per backward
+    key = (x.data_ptr(), tuple(x.shape), stride, groups)
     with _OnWgradStream(x.device, x, g16, dw):
         hit = _COL_CACHE.get(key)
         if hit is not None and hit[2] == x._version:          # (the entry pins the input it was built from: the address cannot be reused)
@@ -691,8 +718,6 @@ def _conv_wgrad_tc(x, g16, w, groups, stride):
                     _COL_CACHE.pop(next(iter(_COL_CACHE)))
                 _COL_CACHE[key] = (x, col, x._version)
         dwp = dw.view(Cout, 9 * Cig) if rows == Cout else torch.empty((rows, 9 * Cig), dtype=torch.float32, device=x.device)
-        ntiles = groups * ((9 * Cig + 127) // 128)
-        splits = 0 if WGRAD_AUTO_SPLIT else max(1, min(128, (2 * 132 + ntiles - 1) // ntiles, M // 256))
         call('tfb_gemm_bf16_tc_wgrad_batched', Cog if groups > 1 else rows, 9 * Cig, M, g16, ldg, Cog if groups > 1 else 0, col, 9 * Cin,
              9 * Cig if groups > 1 else 0, dwp, 9 * Cig, Cog * 9 * Cig, groups, splits)
         if rows != Cout:
@@ -705,12 +730,13 @@ class Conv3x3TCFn(Function):
     TMA tap-shifted NHWC tiles, no im2col); wgrad on the fp32 direct kernel."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, groups, relu, want_stats=False):
+    def forward(ctx, x, w, bias, groups, relu, want_stats=False, implicit_wgrad=False):
         x = _c(x)
         Cout, Cin = w.shape[0], w.shape[1] * groups
         y = _conv_tc_run(_as16(x), w, bias, _conv_tc_plan(Cin, Cout, groups), 0, Cout, groups, relu, want_stats=want_stats)
         ctx.save_for_backward(x, w, y if relu else None, bias)
         ctx.cfg = (groups, relu, bias is not None)
+        ctx.implicit_wgrad = implicit_wgrad
         return y
 
     @staticmethod
@@ -748,7 +774,7 @@ class Conv3x3TCFn(Function):
                 dx = torch.empty_like(x)
                 call('tfb_conv2d_dgrad', g, w, dx, N, H, W, Cin, Cout, 3, 1, groups)
         if ctx.needs_input_grad[1]:
-            dw = _conv_wgrad_tc(x, g16, w, groups, 1) if g16 is not None else None
+            dw = _conv_wgrad_tc(x, g16, w, groups, 1, ctx.implicit_wgrad) if g16 is not None else None
             if dw is not None:
                 if has_bias and db is None:
                     db = _colsum(g.view(-1, Cout), _gbuf(bias_p))
@@ -758,7 +784,7 @@ class Conv3x3TCFn(Function):
                 dw = _gbuf(w)
                 db = (_gbuf(bias_p) if db is None else db) if has_bias else None
                 call('tfb_conv2d_wgrad', x, g, dw, db, N, H, W, Cin, Cout, 3, 1, groups)
-        return dx, dw, db, None, None, None
+        return dx, dw, db, None, None, None, None
 
 
 class Subsample2Fn(Function):
@@ -841,7 +867,8 @@ def max_pool2d(x, emit16=False):
 
 def conv2d(x, w, bias=None, stride=1, groups=1, relu=False, bn_stats=False):
     """bn_stats: a training-mode BatchNorm consumes the result next — on the tensor-core paths (bf16 mode) the producing kernel's
-    epilogue then accumulates the per-channel sum / sum of squares (y._tfb_stats) and batch_norm skips its statistics pass."""
+    epilogue then accumulates the per-channel sum / sum of squares (y._tfb_stats) and batch_norm skips its statistics pass.
+    Inside implicit_wgrad() a 3x3 conv's tensor-core weight gradient skips the im2col matrix (see _conv_wgrad_tc)."""
     if w.shape[2] == 7:
         if not (stride == 2 and groups == 1 and bias is None and not relu and w.shape[1] <= 4):
             raise RuntimeError('7x7 convs are implemented for the ResNet stem only (stride 2, no bias / ReLU, <= 4 input channels)')
@@ -857,9 +884,10 @@ def conv2d(x, w, bias=None, stride=1, groups=1, relu=False, bn_stats=False):
         if st is not None:
             y._tfb_stats = st
         return y
+    implicit = _IMPLICIT_SCOPE[0] > 0
     if G.MODE == 'bf16' and w.shape[2] == 3 and stride == 1 and _conv_tc_plan(w.shape[1] * groups, w.shape[0], groups) is not None:
-        return Conv3x3TCFn.apply(x, w, bias, groups, relu, bn_stats)
-    return Conv2dFn.apply(x, w, bias, stride, groups, relu, bn_stats)
+        return Conv3x3TCFn.apply(x, w, bias, groups, relu, bn_stats, implicit)
+    return Conv2dFn.apply(x, w, bias, stride, groups, relu, bn_stats, implicit)
 
 
 # ------------------------------------------------------------------ normalisation
