@@ -598,7 +598,9 @@ class GeometricFusionBackbone(nn.Module):
         return x
 
     def forward_nhwc(self, image, lidar, bev_points, img_points):
-        """image NCHW 0..255, lidar NCHW, bev_points [B,8,8,5,2] / img_points [B,5,22,5,2] int64 (x, y) correspondences."""
+        """image NCHW 0..255, lidar NCHW, bev_points [B,8,8,5,2] / img_points int64 (x, y) correspondences. img_points is read
+        flat as [B, 5, 22, 5, 2] whatever its shape, as the reference's .view does (geometric_fusion.py:147): the [B,22,5,5,2] the
+        reference's dataset makes (x-major camera cells, data.py:637) is reinterpreted as (h, w) = (5, 22) row-major."""
         cfg = self.config
         if self.training:
             torch._foreach_add_([m.num_batches_tracked for m in self._bn_modules()], 1)
@@ -607,6 +609,8 @@ class GeometricFusionBackbone(nn.Module):
         x = ie.stem.run(ops.image_prep(image), emit16=True)
         l = ops.batch_norm(ops.conv2d(ops.nchw_to_nhwc(lidar), le.conv1.weight, None, 2, 1), le.bn1, True, le.bn1.training, emit16=True)
         ih, iw, lh, lw = cfg.img_vert_anchors, cfg.img_horz_anchors, cfg.lidar_vert_anchors, cfg.lidar_horz_anchors
+        bev_points = bev_points.reshape(bev_points.shape[0], lh, lw, -1, 2)
+        img_points = img_points.reshape(img_points.shape[0], ih, iw, -1, 2)
         prev_lidar_embd = None
         for i in range(1, 5):
             x = getattr(ie, 's%d' % i).run(x, last16=False)

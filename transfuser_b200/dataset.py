@@ -12,7 +12,21 @@ the raw LiDAR sweep, the topdown plane that holds the two BEV channels, and floa
 the frames are cropped and shifted, the sweep is aligned and binned, the target point is drawn, and the BEV label is rotated
 (csrc/bev_label.cu in place of skimage's rotate in load_crop_bev_npy).
 
-Out of scope, and refused: seq_len > 1, the geometric-fusion correspondences, PointPillars, the reference's in-memory cache."""
+Geometric fusion, with the correspondences built on the GPU:
+
+    ds = CarlaRawDataset(roots, TrainConfig(), backbone='geometric_fusion', correspondences='gpu', max_points=40000)
+    tr = Trainer(cfg, 'cuda', backbone='geometric_fusion', raw_inputs='dataset')
+
+The reader does not compute the reference's host-side correspondences (lidar_bev_cam_correspondences, data.py:632-842, with
+its random.sample calls), so backbone='geometric_fusion' alone is refused and correspondences='gpu' opts in: a sample then also
+ships `corr_seed`, drawn with random.getrandbits(63) after the augmentation angle, and the correspondences are built on the GPU
+from the same raw sweep (csrc/correspondences.cu). Cells with at most 5 candidates equal the reference's; in fuller cells the
+seed picks the 5 entries where the reference calls random.sample. Those random.sample calls consume a reference worker's RNG
+state and this draw consumes different state, so the first sample's angle is the reference's but later samples' angles of the
+same worker diverge from a reference worker's.
+
+Out of scope, and refused: seq_len > 1, PointPillars, the reference's host-side correspondences, the reference's in-memory
+cache."""
 import json
 import os
 import random
@@ -92,11 +106,18 @@ def target_point(m, rad):
 
 
 class CarlaRawDataset(torch.utils.data.Dataset):
-    def __init__(self, roots, config, backbone='transFuser', max_points=None):
+    def __init__(self, roots, config, backbone='transFuser', max_points=None, correspondences=None):
         if int(config.seq_len) != 1:
             raise NotImplementedError('CarlaRawDataset reads seq_len == 1 (the reference default) only')
-        if backbone == 'geometric_fusion':
-            raise NotImplementedError('the geometric-fusion correspondences are not produced by CarlaRawDataset')
+        if correspondences not in (None, 'gpu'):
+            raise ValueError("correspondences must be None or 'gpu'")
+        self.geometric = backbone == 'geometric_fusion'
+        if self.geometric and correspondences != 'gpu':
+            raise NotImplementedError("the reference's host-side geometric-fusion correspondences are not produced by CarlaRawDataset; "
+                                      "pass correspondences='gpu' to ship a per-sample seed and build them on the GPU "
+                                      "(InputPipeline.prepare(corr_seed=))")
+        if correspondences == 'gpu' and not self.geometric:
+            raise ValueError("correspondences='gpu' is for backbone='geometric_fusion'")
         if getattr(config, 'use_point_pillars', False):
             raise NotImplementedError('PointPillars inputs are not produced by CarlaRawDataset')
         self.pred_len = int(config.pred_len)
@@ -143,6 +164,7 @@ class CarlaRawDataset(torch.utils.data.Dataset):
         seg = scale_image(_imread(d / 'semantics' / ('%04d.png' % seq), cv2.IMREAD_UNCHANGED), self.scale, nearest=True)
 
         degree = self.draw_degree()
+        corr_seed = random.getrandbits(63) if self.geometric else None    # after the angle: the angle stays the reference's
         rad = np.deg2rad(degree)
         if len(pts) > self.max_points:
             raise ValueError('%s/lidar/%04d.npy holds %d points, more than max_points = %d' % (route, seq, len(pts), self.max_points))
@@ -155,7 +177,7 @@ class CarlaRawDataset(torch.utils.data.Dataset):
         if boxes:
             label[:len(boxes)] = np.array(list(boxes.values()))
         plane = np.ascontiguousarray(top[..., 2])
-        return dict(
+        sample = dict(
             rgb_u8=np.ascontiguousarray(rgb), depth_u8=np.ascontiguousarray(depth), seg_u8=np.ascontiguousarray(seg),
             bev_u8=plane, bev_matrix=pipeline.bev_rotation_matrix(degree, plane.shape[0], plane.shape[1]),
             points=points, n_valid=np.int32(len(pts)),
@@ -163,6 +185,9 @@ class CarlaRawDataset(torch.utils.data.Dataset):
             crop_shift=np.int32(pipeline.crop_shift_pixels(degree, self.img_width, self.scale)),
             target_point64=target_point(m, rad), ego_waypoint=ego_waypoints(labels, rad).astype(np.float32),
             label=label, ego_vel=np.array([m['speed']], dtype=np.float32), degree=np.float64(degree))
+        if corr_seed is not None:
+            sample['corr_seed'] = np.int64(corr_seed)
+        return sample
 
 
 def collate(samples):

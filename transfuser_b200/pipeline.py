@@ -11,7 +11,9 @@ inputs in HBM (csrc/input_prep.cu, csrc/bev_hist.cu):
 
 Host-side pieces that stay numpy, as in the reference (tiny, per sample): the pose algebra of align() (data.py:413-431) and
 the augmentation draw. With the topdown plane and the matrix of bev_rotation_matrix, a fourth launch builds the rotated BEV label
-(csrc/bev_label.cu, skimage's rotate in load_crop_bev_npy). PNG decoding and label parsing stay on the host (dataset.py)."""
+(csrc/bev_label.cu, skimage's rotate in load_crop_bev_npy). With a per-sample seed, a fifth launch builds the geometric-fusion
+LiDAR <-> camera correspondences of the sweep (csrc/correspondences.cu, lidar_bev_cam_correspondences). PNG decoding and label
+parsing stay on the host (dataset.py)."""
 import math
 
 import numpy as np
@@ -60,6 +62,21 @@ def bev_rotation_matrix(degree, H, W):
     return np.array(m[0] + m[1], dtype=np.float64)
 
 
+def correspondence_constants():
+    """The host constants of tfb_lidar_cam_correspondences, from the reference's own numpy expressions: [20] float64 = focal_x,
+    focal_y (data.py:701-706), the left (-60 degrees) and right (+60 degrees) camera rotations row-major (data.py:740-745, 763-768),
+    and the float32 z shift float32(2.5 - 2.3) (data.py:718: a float32 array plus a Python float)."""
+    img_width, img_height, fov_width = 352, 160, 60
+    fov_height = np.rad2deg(2.0 * np.arctan((img_height / img_width) * np.tan(0.5 * np.radians(fov_width))))
+    focal_x = img_width / (2.0 * np.tan(np.deg2rad(fov_width) / 2.0))
+    focal_y = img_height / (2.0 * np.tan(np.deg2rad(fov_height) / 2.0))
+    rot = []
+    for angle in (-60.0, 60.0):
+        theta = np.radians(angle)
+        rot += [np.cos(theta), -np.sin(theta), 0.0, np.sin(theta), np.cos(theta), 0.0, 0.0, 0.0, 1.0]
+    return np.array([focal_x, focal_y] + rot, dtype=np.float64), np.float32(2.5 - 2.3)
+
+
 class InputPipeline:
     def __init__(self, config, device, crop=(160, 704)):
         self.device = torch.device(device)
@@ -70,6 +87,8 @@ class InputPipeline:
             lut[:len(conv)] = np.uint8(conv)
         self.has_lut = conv is not None
         self.lut = torch.from_numpy(lut).to(self.device)
+        consts, self.corr_dz = correspondence_constants()
+        self.corr_consts = torch.from_numpy(consts).to(self.device)
 
     def _require_cuda(self):
         if self.device.type != 'cuda':
@@ -95,11 +114,14 @@ class InputPipeline:
              rgb [B,H,W,3] uint8 (RGB), optional depth [B,H,W,3] uint8, seg [B,H,W] uint8, crop_shift [B] int32 (host values),
              points [B,N,4] float32 (padded), optional n_valid [B] int32, transforms [B,4,4] float64 (align_transform),
              target_point [B,2] float64, optional bev_u8 [B,H,W] uint8 (RGB plane 2 of topdown/encoded_*.png) with bev_matrix
-             [B,6] float64 (bev_rotation_matrix of each sample's augmentation angle).
+             [B,6] float64 (bev_rotation_matrix of each sample's augmentation angle), optional corr_seed [B] int64 >= 0 (the
+             geometric-fusion correspondences of the float32 sweep, data.py:675-842; the seed picks the entries of cells with
+             more than 5 candidates, csrc/correspondences.cu).
            Returns rgb [B,3,h,w] float32 0..255 (or, with normalized_nhwc, the normalised NHWC tensor the backbone consumes
            directly), lidar [B,2,256,256], target_point_image [B,1,256,256], target_point [B,2] float32, and depth [B,h,w] /
            semantic [B,h,w] int64 when their sources are given, and the rotated BEV label bev [B,160,160] int64
-           (load_crop_bev_npy, csrc/bev_label.cu) when bev_u8 is given. `out` (optional dict) supplies preallocated destinations
+           (load_crop_bev_npy, csrc/bev_label.cu) when bev_u8 is given, and bev_points [B,8,8,5,2] / cam_points [B,22,5,5,2] int64
+           when corr_seed is given. `out` (optional dict) supplies preallocated destinations
            by the same keys, so the three launches can write straight into the static inputs of a captured training step."""
         self._require_cuda()
         res = {}
@@ -170,4 +192,17 @@ class InputPipeline:
             bev_out = self._out(out, 'bev', (B, 160, 160), torch.int64)
             _lib.call('tfb_bev_label_prep', plane, m, B, plane.shape[1], plane.shape[2], bev_out)
             res['bev'] = bev_out
+
+        if raw.get('corr_seed') is not None:
+            if points.dtype != torch.float32:
+                raise ValueError('the correspondences read a float32 sweep (the dtype dataset.CarlaRawDataset ships)')
+            seed = self._dev(raw['corr_seed'], torch.int64)
+            if tuple(seed.shape) != (B,):
+                raise ValueError('corr_seed must be [B] int64, got %s' % (tuple(seed.shape),))
+            N = points.shape[1]
+            work = torch.empty((B, 6 * max(N, 1)), dtype=torch.int32, device=self.device)
+            bev_pts = self._out(out, 'bev_points', (B, 8, 8, 5, 2), torch.int64)
+            cam_pts = self._out(out, 'cam_points', (B, 22, 5, 5, 2), torch.int64)
+            _lib.call('tfb_lidar_cam_correspondences', points, n_valid, seed, self.corr_consts, float(self.corr_dz), B, N, work, bev_pts, cam_pts)
+            res['bev_points'], res['cam_points'] = bev_pts, cam_pts
         return res

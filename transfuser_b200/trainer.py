@@ -27,11 +27,14 @@ class Trainer:
     def __init__(self, cfg, device, gemm_mode='bf16', lr=1e-4, seed=0, n_chunks=int(os.environ.get('TFB_GRAD_CHUNKS', '8')), backbone='transFuser',
                  raw_inputs=False, image_architecture='regnety_032', lidar_architecture='regnety_032'):
         self.cfg, self.device = cfg, device
-        # the geometric-fusion backbone consumes two more inputs per sample (train.py:279-288)
         self.raw_inputs = raw_inputs
         if raw_inputs not in (False, True, 'dataset'):
             raise ValueError("raw_inputs must be False, True or 'dataset'")
-        self.input_keys = (DATASET_KEYS if raw_inputs == 'dataset' else RAW_KEYS if raw_inputs else INPUT_KEYS) + (('bev_points', 'cam_points') if backbone == 'geometric_fusion' else ())
+        # the geometric-fusion backbone consumes two more inputs per sample, the LiDAR <-> camera correspondences
+        # (train.py:279-288); in dataset mode they are built inside the step from the sweep and a per-sample seed (csrc/correspondences.cu)
+        geo = backbone == 'geometric_fusion'
+        self.input_keys = (DATASET_KEYS + (('corr_seed',) if geo else ()) if raw_inputs == 'dataset' else
+                           (RAW_KEYS if raw_inputs else INPUT_KEYS) + (('bev_points', 'cam_points') if geo else ()))
         if raw_inputs:
             from .pipeline import InputPipeline
             self.pipe = InputPipeline(cfg, device)
@@ -92,9 +95,12 @@ class Trainer:
                        transforms=d['transforms'], target_point=d['target_point64'])
             if self.raw_inputs == 'dataset':
                 raw.update(n_valid=d['n_valid'], bev_u8=d['bev_u8'], bev_matrix=d['bev_matrix'])   # + the BEV-label rotation
+                if 'corr_seed' in d:
+                    raw['corr_seed'] = d['corr_seed']                                                # + the correspondences
             p = self.pipe.prepare(raw, normalized_nhwc=True)
             d = dict(d, rgb=p['rgb'], depth=p['depth'], semantic=p['semantic'], target_point=p['target_point'],
-                     target_point_image=p['target_point_image'], bev=p.get('bev', d.get('bev')))
+                     target_point_image=p['target_point_image'], bev=p.get('bev', d.get('bev')),
+                     bev_points=p.get('bev_points', d.get('bev_points')), cam_points=p.get('cam_points', d.get('cam_points')))
             lidar = p['lidar']
         else:
             lidar = bev.lidar_to_histogram_features_batched(d['points'])
