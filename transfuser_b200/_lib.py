@@ -112,7 +112,8 @@ class Profiler:
     FAMILY = {'tfb_gemm_bf16_tc': 'gemm_tc_kernel', 'tfb_gemm_bf16_tc_stats': 'gemm_tc_kernel', 'tfb_gemm_bf16_tc_out16': 'gemm_tc_kernel',
               'tfb_gemm_bf16_tc_wgrad_batched': 'gemm_tc_kernel', 'tfb_conv3x3_tc': 'conv3x3_tc_kernel', 'tfb_conv3x3_tc_strided': 'conv3x3_tc_kernel',
               'tfb_bn_fwd': 'bn_fwd (colreduce4 + bn_apply)', 'tfb_bn_fwd_stats': 'bn_apply_stats_kernel', 'tfb_attn_fwd_tc': 'attn_tc_kernel',
-              'tfb_attn_bwd_tc': 'attn_tc_kernel', 'tfb_conv3x3_tc_wgrad': 'gemm_tc_kernel'}
+              'tfb_attn_bwd_tc': 'attn_tc_kernel', 'tfb_conv3x3_tc_wgrad': 'gemm_tc_kernel', 'tfb_gemm_bf16_tc_bn_eval': 'gemm_tc_kernel',
+              'tfb_conv3x3_tc_bn_eval': 'conv3x3_tc_kernel'}
 
     def __init__(self, keep_calls=False):
         self.records = []

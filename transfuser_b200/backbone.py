@@ -20,7 +20,12 @@ RESNET_WIDTHS = (64, 128, 256, 512)
 
 
 def _conv_bn(conv, bn, x, stride=1, groups=1, act=True, emit16=False, residual=None, pool=False):
-    """bn(conv(x)) with the ReLU (act), the residual add and the SE pool fused into the BatchNorm passes (see _ConvBn.run)."""
+    """bn(conv(x)) with the ReLU (act), the residual add and the SE pool fused into the BatchNorm passes (see _ConvBn.run). An
+    eval-mode BatchNorm runs inside the tensor-core conv's epilogue where there is one (ops.conv_bn_eval)."""
+    if not bn.training:
+        y = ops.conv_bn_eval(x, conv.weight, bn, stride, groups, act or residual is not None, residual, emit16)
+        if y is not None:
+            return y
     y = ops.conv2d(x, conv.weight, None, stride, groups, bn_stats=bn.training)
     # bwd16: this conv has no bias / ReLU of its own, so BatchNorm's dx is exactly the dy its tensor-core dgrad / wgrad read
     return ops.batch_norm(y, bn, act or residual is not None, bn.training, emit16, bwd16=conv.in_channels % 8 == 0, residual=residual,
@@ -403,6 +408,7 @@ class TransfuserBackbone(nn.Module):
             main = torch.cuda.current_stream()
             side = ops.side_stream(image.device)
             side.wait_stream(main)
+            ops.record_stream(l, side)      # made on main, read on side: without autograd holding it (eval) it is freed right after
             with torch.cuda.stream(side):
                 l = le.run_stem(l)
             x = ie.run_stem(x)
@@ -499,6 +505,7 @@ class LateFusionBackbone(nn.Module):
             main, side = torch.cuda.current_stream(), ops.side_stream(image.device)
             l = ops.nchw_to_nhwc(lidar)
             side.wait_stream(main)
+            ops.record_stream(l, side)      # made on main, read on side: without autograd holding it (eval) it is freed right after
             with torch.cuda.stream(side):
                 l = self.lidar_encoder.run(l)
             x = self.image_encoder.run(ops.image_prep(image))

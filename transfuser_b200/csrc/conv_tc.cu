@@ -19,12 +19,12 @@ constexpr int TH = 8, TW = 16, BM = TH * TW;
 constexpr int kThreads = 288;                   // warps 0-7: two consumer warpgroups (tile rows 0-3 / 4-7); warp 8: TMA producer
 constexpr int kStageFloats = 16 * 36;           // one warp's epilogue staging block
 
-template <int KC, int NB, int STAGES>
+template <int KC, int NB, int STAGES, bool BNE = false>
 __global__ void __launch_bounds__(kThreads, NB <= 64 ? 2 : 1)
 conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constant__ CUtensorMap tma_w, float* __restrict__ y,
                   const float* __restrict__ bias, int H, int W, int Cout, int tiles_w, int tiles_h, int c_step, int nchunks,
                   int nb_real, int relu, int gblocks, int total_tiles, int stride, double* __restrict__ stats, float* __restrict__ ws,
-                  unsigned int* __restrict__ ws_cnt) {
+                  unsigned int* __restrict__ ws_cnt, const tc::BnEval bne, __nv_bfloat16* __restrict__ y16) {
   // H, W: OUTPUT height / width. stride 2: the activation map steps two pixels per box element, so tile pixel (h, w) reads the
   // input pixel (2h + dy, 2w + dx) of tap (dy, dx).
   // PERSISTENT: tile t = (spatial tile, channel block), channel block fastest (CTAs running together re-use the same activation
@@ -111,7 +111,8 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_consta
       const int nvalid = min(nb_real, Cout - gb * nb_real);
       float* ytile = y + (int64_t)gb * nb_real;
       const float* bp = bias ? bias + gb * nb_real : nullptr;
-      const bool fast = (Cout & 3) == 0 && ((gb * nb_real) & 3) == 0 && ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
+      // BNE: the host checked the alignments of the coalesced path
+      const bool fast = BNE || ((Cout & 3) == 0 && ((gb * nb_real) & 3) == 0 && ((reinterpret_cast<uintptr_t>(y) & 15) == 0));
       if (fast) {
 #pragma unroll
         for (int c = 0; c < (NB + 31) / 32; ++c) {
@@ -119,17 +120,24 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_consta
           const int cols_valid = min(nvalid - c0, NB - c0);
           if (cols_valid <= 0) break;
           tc::frag_to_stage(stage, acc, c, lane);
-          tc::stage_to_global(stage,
-                              [=](int row) -> int64_t {
-                                const int w = w0 + row;
-                                return (h < H && w < W) ? (((int64_t)n * H + h) * W + w) * Cout + c0 : (int64_t)-1;
-                              },
-                              cols_valid, bp ? bp + c0 : nullptr, 1.f, relu, lane, ytile, nullptr,
-                              stats ? wstat + (warp * 2) * tc::kStatW + c0 : nullptr,
-                              stats ? wstat + (warp * 2 + 1) * tc::kStatW + c0 : nullptr);
+          auto row_off = [=](int row) -> int64_t {
+            const int w = w0 + row;
+            return (h < H && w < W) ? (((int64_t)n * H + h) * W + w) * Cout + c0 : (int64_t)-1;
+          };
+          if constexpr (BNE) {
+            const int cb = gb * nb_real + c0;
+            const tc::BnEval b{bne.mean + cb, bne.invstd + cb, bne.gamma + cb, bne.beta + cb, bne.res ? bne.res + gb * nb_real : nullptr,
+                               bne.relu};
+            tc::stage_to_global<true>(stage, row_off, cols_valid, nullptr, 1.f, 0, lane, ytile, y16 ? y16 + gb * nb_real : nullptr, nullptr,
+                                      nullptr, 0, &b);
+          } else {
+            tc::stage_to_global(stage, row_off, cols_valid, bp ? bp + c0 : nullptr, 1.f, relu, lane, ytile, nullptr,
+                                stats ? wstat + (warp * 2) * tc::kStatW + c0 : nullptr,
+                                stats ? wstat + (warp * 2 + 1) * tc::kStatW + c0 : nullptr);
+          }
         }
         if (stats) tc::stat_fold(s_stat, wstat, Cout, gb * nb_real, nvalid, (int)threadIdx.x);
-      } else {
+      } else if constexpr (!BNE) {
         const int t128 = threadIdx.x & 127;
 #pragma unroll
         for (int i = 0; i < NB / 2; ++i) {
@@ -151,7 +159,8 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_consta
 
 template <int KC, int NB>
 int launch_conv(const void* x16, const void* wpack, const float* bias, float* y, int N, int Hin, int Win, int Cx, int Cy, int c_step,
-                int nchunks, int nb_real, int gblocks, int relu, int stride, double* stats, cudaStream_t stream) {
+                int nchunks, int nb_real, int gblocks, int relu, int stride, double* stats, cudaStream_t stream,
+                const tc::BnEval* bne = nullptr, __nv_bfloat16* y16 = nullptr) {
   const int H = (Hin - 1) / stride + 1, W = (Win - 1) / stride + 1;       // output size (kernel 3, pad 1)
   constexpr int STAGES = NB <= 64 ? 6 : 4;
   constexpr int STAGE = BM * KC * 2 + NB * KC * 2;
@@ -175,11 +184,11 @@ int launch_conv(const void* x16, const void* wpack, const float* bias, float* y,
     tfb_set_last_error("cuTensorMapEncodeTiled(packed weights) failed");
     return TFB_ERR_DRIVER;
   }
-  auto kern = conv3x3_tc_kernel<KC, NB, STAGES>;
-  static bool attr_done = false;
-  if (!attr_done) {
+  auto kern = bne ? conv3x3_tc_kernel<KC, NB, STAGES, true> : conv3x3_tc_kernel<KC, NB, STAGES>;
+  static bool attr_done[2] = {false, false};
+  if (!attr_done[bne ? 1 : 0]) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM0 + (2 * 2048 + 8 * 2 * tc::kStatW) * (int)sizeof(float)) != cudaSuccess) return TFB_ERR_DRIVER;
-    attr_done = true;
+    attr_done[bne ? 1 : 0] = true;
   }
   const int tiles_w = (W + TW - 1) / TW, tiles_h = (H + TH - 1) / TH;
   const int64_t total = (int64_t)tiles_w * tiles_h * N * gblocks;
@@ -195,7 +204,7 @@ int launch_conv(const void* x16, const void* wpack, const float* bias, float* y,
     if (rc != TFB_OK) return rc;
   }
   kern<<<grid, kThreads, SMEM, stream>>>(mx, mw, y, bias, H, W, Cy, tiles_w, tiles_h, c_step, nchunks, nb_real, relu, gblocks, (int)total, stride, stats,
-                                         wk.f, wk.cnt);
+                                         wk.f, wk.cnt, bne ? *bne : tc::BnEval{}, y16);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
@@ -225,4 +234,26 @@ TFB_API int tfb_conv3x3_tc_strided(const void* x16, const void* wpack, const flo
 TFB_API int tfb_conv3x3_tc(const void* x16, const void* wpack, const float* bias, float* y, int N, int H, int W, int Cx, int Cy,
                            int NB, int KC, int c_step, int nchunks, int nb_real, int gblocks, int relu, cudaStream_t stream) {
   return tfb_conv3x3_tc_strided(x16, wpack, bias, y, N, H, W, Cx, Cy, NB, KC, c_step, nchunks, nb_real, gblocks, relu, 1, nullptr, stream);
+}
+
+// Eval-mode BatchNorm behind a 3x3 conv (stride 1 or 2) in one launch: y = relu?( fma((conv - mean) * invstd, gamma, beta) + residual ),
+// and, when y16 is given, its bf16 copy (round-to-nearest-even, y's layout). The tile plan and the arguments of the conv are those of
+// tfb_conv3x3_tc_strided (no bias, no ReLU, no statistics of the conv itself); per element, the operations of tfb_bn_apply on that
+// launch's output, so the same bits as the two launches. invstd = 1 / sqrt(running_var + eps), computed by the caller. residual
+// (optional): fp32 with y's layout. Cy % 4 == 0 and nb_real % 4 == 0; y and the residual 16-byte aligned, y16 8-byte aligned.
+TFB_API int tfb_conv3x3_tc_bn_eval(const void* x16, const void* wpack, float* y, int N, int H, int W, int Cx, int Cy, int NB, int KC,
+                                   int c_step, int nchunks, int nb_real, int gblocks, int stride, const float* mean, const float* invstd,
+                                   const float* gamma, const float* beta, const float* residual, int relu, void* y16, cudaStream_t stream) {
+  TFB_REQUIRE(x16 && wpack && y && N > 0 && H > 0 && W > 0 && Cx > 0 && Cy > 0 && Cx % 8 == 0 && (stride == 1 || stride == 2));
+  TFB_REQUIRE(mean && invstd && gamma && beta && Cy % 4 == 0 && nb_real % 4 == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0);
+  TFB_REQUIRE((reinterpret_cast<uintptr_t>(residual) & 15) == 0 && (reinterpret_cast<uintptr_t>(y16) & 7) == 0);
+  TFB_REQUIRE((reinterpret_cast<uintptr_t>(x16) & 15) == 0 && (reinterpret_cast<uintptr_t>(wpack) & 15) == 0);
+  const tc::BnEval bne{mean, invstd, gamma, beta, residual, relu ? 1 : 0};
+  __nv_bfloat16* o16 = (__nv_bfloat16*)y16;
+#define CASE(KC_, NB_) if (KC == KC_ && NB == NB_) return launch_conv<KC_, NB_>(x16, wpack, nullptr, y, N, H, W, Cx, Cy, c_step, nchunks, nb_real, gblocks, 0, stride, nullptr, stream, &bne, o16)
+  CASE(64, 16); CASE(64, 32); CASE(64, 48); CASE(64, 64); CASE(64, 128);
+  CASE(32, 16); CASE(32, 32); CASE(32, 64);
+#undef CASE
+  tfb_set_last_error("tfb_conv3x3_tc_bn_eval: unsupported (KC, NB) tile");
+  return TFB_ERR_UNSUPPORTED;
 }

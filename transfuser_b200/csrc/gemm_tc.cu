@@ -58,13 +58,13 @@ struct ConvGather {
 
 constexpr int kGatherThreads = kThreads + 96;                 // GATHER: warps 8-11 produce (168 registers x 384 threads fit)
 
-template <typename T, bool A_MN, bool B_MN, int BN, bool GATHER = false>
+template <typename T, bool A_MN, bool B_MN, int BN, bool GATHER = false, bool BNE = false>
 __global__ void __launch_bounds__(GATHER ? kGatherThreads : kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, float* __restrict__ Cbase,
                int64_t ldc, int M, int N, int num_kb, int kb_per_split, const float* __restrict__ bias, float alpha, float beta,
                int relu, int atomic_out, int splits, int a_step, int b_step, int64_t c_bstride, int tiles_m, int tiles_n,
                int total_tiles, int STAGES, double* __restrict__ stats, __nv_bfloat16* __restrict__ C16, float* __restrict__ ws,
-               unsigned int* __restrict__ ws_cnt, const ConvGather cg) {
+               unsigned int* __restrict__ ws_cnt, const ConvGather cg, const tc::BnEval bne) {
   // PERSISTENT: gridDim.x CTAs (<= one per SM) walk the tile list t = blockIdx.x, += gridDim.x. A tile is (m-tile, n-tile, z),
   // z = batch * splits + split; m fastest so that concurrently running CTAs share the same B (weight) tile in L2.
   // Consumer warpgroup g (warps 4g..4g+3) owns rows [64g, 64g + 64) of the 128 x BN tile as a wgmma register accumulator;
@@ -269,8 +269,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         continue;
       }
       float* cwarp = Cbase + (int64_t)bz * c_bstride + (int64_t)r0 * ldc;
-      const bool fast = (atomic_out || beta == 0.f) && (ldc & 3) == 0 &&
-                        (C16 ? (reinterpret_cast<uintptr_t>(C16) & 7) == 0 : (reinterpret_cast<uintptr_t>(cwarp + n0) & 15) == 0);
+      // BNE: the host checked the alignments of the coalesced path (C, residual and C16 are all written / read there)
+      const bool fast = BNE || ((atomic_out || beta == 0.f) && (ldc & 3) == 0 &&
+                                (C16 ? (reinterpret_cast<uintptr_t>(C16) & 7) == 0 : (reinterpret_cast<uintptr_t>(cwarp + n0) & 15) == 0));
       if (fast) {
         // coalesced path: 32-column chunks through this warp's padded smem staging buffer
         float* stage = stage_out + warp * kStageFloats;
@@ -282,13 +283,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           if (cols_valid <= 0) break;   // warp-uniform
           const int64_t off0 = (int64_t)bz * c_bstride + (int64_t)r0 * ldc + n0 + c0;
           tc::frag_to_stage(stage, acc, c, lane);
-          tc::stage_to_global(stage, [=](int row) -> int64_t { return row < rows_valid ? off0 + (int64_t)row * ldc : (int64_t)-1; },
-                              cols_valid, add_bias ? bias + n0 + c0 : nullptr, alpha, relu, lane, Cbase, C16,
-                              stats ? wstat + (warp * 2) * tc::kStatW + c0 : nullptr,
-                              stats ? wstat + (warp * 2 + 1) * tc::kStatW + c0 : nullptr, atomic_out);
+          auto row_off = [=](int row) -> int64_t { return row < rows_valid ? off0 + (int64_t)row * ldc : (int64_t)-1; };
+          if constexpr (BNE) {
+            const int cb = n0 + c0;
+            const tc::BnEval b{bne.mean + cb, bne.invstd + cb, bne.gamma + cb, bne.beta + cb, bne.res, bne.relu};
+            tc::stage_to_global<true>(stage, row_off, cols_valid, nullptr, alpha, 0, lane, Cbase, C16, nullptr, nullptr, 0, &b);
+          } else {
+            tc::stage_to_global(stage, row_off, cols_valid, add_bias ? bias + n0 + c0 : nullptr, alpha, relu, lane, Cbase, C16,
+                                stats ? wstat + (warp * 2) * tc::kStatW + c0 : nullptr,
+                                stats ? wstat + (warp * 2 + 1) * tc::kStatW + c0 : nullptr, atomic_out);
+          }
         }
         if (stats) tc::stat_fold(s_stat, wstat, N, n0, min(BN, N - n0), (int)threadIdx.x);
-      } else {
+      } else if constexpr (!BNE) {
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) {
           const int m = m0 + wg * 64 + tc::frag_row(t128, i), n = n0 + tc::frag_col(t128, i);
@@ -346,7 +353,8 @@ bool make_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols,
 template <typename T, bool A_MN, bool B_MN, int BN>
 int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
               int relu, float alpha, float beta, int splits, cudaStream_t stream, int nbatch = 1, int a_step = 0, int b_step = 0,
-              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr, const ConvGather* gather = nullptr) {
+              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr, const ConvGather* gather = nullptr,
+              const tc::BnEval* bne = nullptr) {
   using E = Elem<T>;
   if (C16) {     // bf16 output: coalesced epilogue path only
     TFB_REQUIRE(splits <= 1 && beta == 0.f && (ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(C16) & 7) == 0);
@@ -389,13 +397,18 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
     if (gather) kern = gemm_tc_kernel<T, A_MN, B_MN, BN, true>;
   }
   if (gather && kern == gemm_tc_kernel<T, A_MN, B_MN, BN>) { tfb_set_last_error("gathered B: bf16 wgrad form only"); return TFB_ERR_UNSUPPORTED; }
-  static bool attr_done[2] = {false, false};
-  if (!attr_done[gather ? 1 : 0]) {
+  if constexpr (sizeof(T) == 2 && !A_MN && !B_MN) {
+    if (bne) kern = gemm_tc_kernel<T, A_MN, B_MN, BN, false, true>;
+  }
+  if (bne && kern == gemm_tc_kernel<T, A_MN, B_MN, BN>) { tfb_set_last_error("eval-mode BatchNorm epilogue: bf16 y = x W^T form only"); return TFB_ERR_UNSUPPORTED; }
+  const int variant = gather ? 1 : bne ? 2 : 0;
+  static bool attr_done[3] = {false, false, false};
+  if (!attr_done[variant]) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) != cudaSuccess) {
       tfb_set_last_error("cudaFuncSetAttribute(smem) failed");
       return TFB_ERR_DRIVER;
     }
-    attr_done[gather ? 1 : 0] = true;
+    attr_done[variant] = true;
   }
   const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
   const int64_t total = (int64_t)tiles_m * tiles_n * splits * nbatch;
@@ -417,7 +430,7 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
   }
   kern<<<grid, gather ? kGatherThreads : kThreads, smem_total, stream>>>(ma, mb, C, ldc, M, N, num_kb, kb_per_split, bias, alpha, beta, relu, atomic_out, splits,
                                                a_step, b_step, c_bstride, tiles_m, tiles_n, (int)total, stages, stats, C16, ws.f,
-                                               post_fold ? nullptr : ws.cnt, gather ? *gather : ConvGather{});
+                                               post_fold ? nullptr : ws.cnt, gather ? *gather : ConvGather{}, bne ? *bne : tc::BnEval{});
   TFB_CHECK_LAUNCH();
   if (post_fold) {
     const int64_t n_out = (int64_t)M * N, groups = n_out % 4 == 0 ? n_out / 4 : n_out;
@@ -431,9 +444,10 @@ int launch_bn(int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t 
 template <typename T, bool A_MN, bool B_MN>
 int launch_tc(int BN, int M, int N, int K, const T* A, int64_t lda, const T* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
               int relu, float alpha, float beta, int splits, cudaStream_t stream, int nbatch = 1, int a_step = 0, int b_step = 0,
-              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr, const ConvGather* gather = nullptr) {
+              int64_t c_bstride = 0, double* stats = nullptr, __nv_bfloat16* C16 = nullptr, const ConvGather* gather = nullptr,
+              const tc::BnEval* bne = nullptr) {
 #define TFB_BN(bn_) case bn_: return launch_bn<T, A_MN, B_MN, bn_>(M, N, K, A, lda, B, ldb, C, ldc, bias, relu, alpha, beta, splits, stream, \
-                                                                  nbatch, a_step, b_step, c_bstride, stats, C16, gather)
+                                                                  nbatch, a_step, b_step, c_bstride, stats, C16, gather, bne)
   if constexpr (B_MN) {
     switch (BN) { TFB_BN(64); TFB_BN(128); TFB_BN(192); }
   } else {
@@ -620,6 +634,25 @@ TFB_API int tfb_gemm_bf16_tc_out16(int transB, int M, int N, int K, const void* 
   TFB_REQUIRE(C16 != nullptr);
   return gemm_tc_any<__nv_bfloat16>(0, transB, M, N, K, (const __nv_bfloat16*)A, lda, (const __nv_bfloat16*)B, ldb, nullptr, ldc, bias, relu,
                                     alpha, 0.f, 1, stream, nullptr, (__nv_bfloat16*)C16);
+}
+
+// Eval-mode BatchNorm behind a 1x1 conv / linear layer in one launch: C[M,N] (fp32, row stride ldc) =
+//   relu?( fma((x W^T - mean) * invstd, gamma, beta) + residual ),  x[M,K], W[N,K] bf16, residual (optional) fp32 with C's layout,
+// and, when C16 is given, its bf16 copy (round-to-nearest-even, same layout). The same tile plan as tfb_gemm_bf16_tc(0, 1, ..., splits 1)
+// and, per element, the operations of tfb_bn_apply on that launch's output: the same bits as the two launches, without the
+// unnormalised product ever reaching memory. invstd = 1 / sqrt(running_var + eps), computed by the caller. N % 4 == 0, ldc % 4 == 0;
+// C and the residual 16-byte aligned, C16 8-byte aligned.
+TFB_API int tfb_gemm_bf16_tc_bn_eval(int M, int N, int K, const void* A, int64_t lda, const void* B, int64_t ldb, float* C, int64_t ldc,
+                                     const float* mean, const float* invstd, const float* gamma, const float* beta, const float* residual,
+                                     int relu, void* C16, cudaStream_t stream) {
+  TFB_REQUIRE(M > 0 && N > 0 && K > 0 && A && B && C && mean && invstd && gamma && beta);
+  TFB_REQUIRE(N % 4 == 0 && ldc % 4 == 0 && ldc >= N && (reinterpret_cast<uintptr_t>(C) & 15) == 0);
+  TFB_REQUIRE((reinterpret_cast<uintptr_t>(residual) & 15) == 0 && (reinterpret_cast<uintptr_t>(C16) & 7) == 0);
+  TFB_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0 && lda % 8 == 0 && ldb % 8 == 0);
+  using T = __nv_bfloat16;
+  const tc::BnEval bne{mean, invstd, gamma, beta, residual, relu ? 1 : 0};
+  return launch_tc<T, false, false>(pick_bn(M, N, 1, 32), M, N, K, (const T*)A, lda, (const T*)B, ldb, C, ldc, nullptr, 0, 1.f, 0.f, 1, stream,
+                                    1, 0, 0, 0, nullptr, (T*)C16, nullptr, &bne);
 }
 
 // Caps the persistent grid of the following tensor-core GEMM launches at max_ctas CTAs (0 = no cap: one per SM). The weight-gradient

@@ -319,6 +319,20 @@ __global__ void ratio_kernel(const double* __restrict__ num, const double* __res
   *out = (float)v;
 }
 
+// One validation batch of the reference's Engine.validate (train.py:333-340), operation for operation: for k < n (the model's loss
+// dict order), wv = w_k * loss_k in fp32, acc[k] += (double)wv; the batch total is the fp32 running sum 0 + wv_0 + wv_1 + ...,
+// then acc[n] += (double)total; acc[n + 1] += 1 (the batch count). One thread: n is 11.
+__global__ void val_accumulate_kernel(const int64_t* __restrict__ loss_ptrs, const float* __restrict__ w, int n, double* __restrict__ acc) {
+  float total = 0.f;
+  for (int k = 0; k < n; ++k) {
+    const float wv = __fmul_rn(w[k], *reinterpret_cast<const float*>(loss_ptrs[k]));
+    acc[k] += (double)wv;
+    total = __fadd_rn(total, wv);
+  }
+  acc[n] += (double)total;
+  acc[n + 1] += 1.0;
+}
+
 }  // namespace
 
 TFB_API int tfb_ce_fwd(const float* logits, const int64_t* target, int64_t M, int C, const float* class_w, const float* pos_w, int HW,
@@ -390,6 +404,16 @@ TFB_API int tfb_centernet_loss_bwd(const float* pred, const float* tgt, int B, i
                                    float* dpred, cudaStream_t stream) {
   TFB_REQUIRE(pred && tgt && count && gout7 && dpred && B > 0 && HW > 0);
   centernet_loss_kernel<1><<<tfb_grid((int64_t)B * HW, 256, 2), 256, 0, stream>>>(pred, tgt, B, HW, count, nullptr, gout7, dpred);
+  TFB_CHECK_LAUNCH();
+  return TFB_OK;
+}
+
+// Validation bookkeeping of one batch without a host read-back: loss_ptrs[k] (device int64 table) is the address of the fp32 scalar
+// loss k, weights[k] its fp32 weight, acc[n + 2] fp64 (n weighted sums, the total, the batch count; zeroed by the caller once per
+// validation). See val_accumulate_kernel.
+TFB_API int tfb_val_accumulate(const int64_t* loss_ptrs, const float* weights, int n, double* acc, cudaStream_t stream) {
+  TFB_REQUIRE(loss_ptrs && weights && acc && n > 0);
+  val_accumulate_kernel<<<1, 1, 0, stream>>>(loss_ptrs, weights, n, acc);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }

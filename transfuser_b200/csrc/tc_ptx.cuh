@@ -107,6 +107,22 @@ __device__ __forceinline__ void frag_to_stage(float* stage, const float (&acc)[K
   __syncwarp();
 }
 
+// Eval-mode BatchNorm in the epilogue (tfb_gemm_bf16_tc_bn_eval, tfb_conv3x3_tc_bn_eval): every pointer is pre-offset to the chunk's
+// column 0 (res: to the output's base, like out32). o = fma((v - mean) * invstd, gamma, beta) (+ res) (ReLU), v being the value
+// the plain launch stores: the same operations, in the same order and without contraction, as bn_apply_kernel (norm.cu).
+struct BnEval {
+  const float* mean;
+  const float* invstd;
+  const float* gamma;
+  const float* beta;
+  const float* res;     // optional residual with the output's layout
+  int relu;
+};
+
+__device__ __forceinline__ float bn_eval_one(float v, float mu, float is, float ga, float be) {
+  return fmaf(__fmul_rn(__fsub_rn(v, mu), is), ga, be);
+}
+
 // Epilogue, part 2: one warp writes the 16 x 32 staged block to global memory with COALESCED row segments (4 rows per
 // instruction, 128 bytes of fp32 or 64 bytes of bf16 per row), applying o = alpha*acc + bias (ReLU).
 // `row_off(row)` returns the ELEMENT offset of staged row `row` (0..15) in the output (a multiple of 4) or -1 for rows that
@@ -117,10 +133,13 @@ __device__ __forceinline__ void frag_to_stage(float* stage, const float (&acc)[K
 // output come out of its epilogue instead of a separate read pass over the tensor. They are STORED (each column of a tile belongs
 // to one chunk); stat_fold adds the warps' buffers into the CTA's accumulators in warp order, and stat_flush reduces the CTAs in
 // CTA order, so the statistics are the same bits on every run.
-template <class RowOff>
+// BNE (eval-mode BatchNorm, `bne` set): the normalised value goes to out32 AND, when out16 is given, to out16; no atomic, no
+// statistics.
+template <bool BNE = false, class RowOff>
 __device__ __forceinline__ void stage_to_global(const float* stage, RowOff row_off, int cols_valid, const float* bias, float alpha,
                                                 int relu, int lane, float* out32, __nv_bfloat16* out16 = nullptr,
-                                                float* stat_sum = nullptr, float* stat_sq = nullptr, int atomic = 0) {
+                                                float* stat_sum = nullptr, float* stat_sq = nullptr, int atomic = 0,
+                                                const BnEval* bne = nullptr) {
   const int c4 = (lane & 7) * 4, rsub = lane >> 3;
   float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
   if (bias) {
@@ -137,6 +156,53 @@ __device__ __forceinline__ void stage_to_global(const float* stage, RowOff row_o
     v.x = fmaf(alpha, v.x, bv.x); v.y = fmaf(alpha, v.y, bv.y); v.z = fmaf(alpha, v.z, bv.z); v.w = fmaf(alpha, v.w, bv.w);
     if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
     const int64_t off = row_off(row);
+    if constexpr (BNE) {
+      if (off >= 0) {
+        // the per-channel parameters are re-read per row (L1 hits): held across the rows they push the 96-register tiles into spills
+        float* vq = &v.x;
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          if (c4 + q < cols_valid) vq[q] = bn_eval_one(vq[q], bne->mean[c4 + q], bne->invstd[c4 + q], bne->gamma[c4 + q], bne->beta[c4 + q]);
+        const bool full = c4 + 3 < cols_valid;
+        if (bne->res) {
+          const float* r = bne->res + off + c4;
+          float4 rv;
+          if (full) {
+            rv = *reinterpret_cast<const float4*>(r);
+          } else {
+            rv.x = c4 + 0 < cols_valid ? r[0] : 0.f;
+            rv.y = c4 + 1 < cols_valid ? r[1] : 0.f;
+            rv.z = c4 + 2 < cols_valid ? r[2] : 0.f;
+            rv.w = 0.f;
+          }
+          v.x = __fadd_rn(v.x, rv.x); v.y = __fadd_rn(v.y, rv.y); v.z = __fadd_rn(v.z, rv.z); v.w = __fadd_rn(v.w, rv.w);
+        }
+        if (bne->relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+        float* p = out32 + off + c4;
+        if (full) {
+          *reinterpret_cast<float4*>(p) = v;
+        } else {
+          if (c4 + 0 < cols_valid) p[0] = v.x;
+          if (c4 + 1 < cols_valid) p[1] = v.y;
+          if (c4 + 2 < cols_valid) p[2] = v.z;
+        }
+        if (out16) {
+          __nv_bfloat16* p16 = out16 + off + c4;
+          if (full) {
+            __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+            uint2 o;
+            o.x = *reinterpret_cast<uint32_t*>(&lo);
+            o.y = *reinterpret_cast<uint32_t*>(&hi);
+            *reinterpret_cast<uint2*>(p16) = o;
+          } else {
+            if (c4 + 0 < cols_valid) p16[0] = __float2bfloat16_rn(v.x);
+            if (c4 + 1 < cols_valid) p16[1] = __float2bfloat16_rn(v.y);
+            if (c4 + 2 < cols_valid) p16[2] = __float2bfloat16_rn(v.z);
+          }
+        }
+      }
+      continue;
+    }
     if (off >= 0) {
       if (stat_sum) {
         s1[0] += v.x; s1[1] += v.y; s1[2] += v.z; s1[3] += v.w;

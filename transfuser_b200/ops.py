@@ -646,13 +646,19 @@ def _prepack_all(device):
         e.epoch, e.version = _PACK_STATE['epoch'], w._version
 
 
-def _conv_tc_run(x16, w, bias, plan, mode, c_write, groups, relu, stride=1, want_stats=False):
-    N, H, W, c_read = x16.shape
+def _packed_current(w, plan, mode, groups):
+    """The packed buffer of (w, mode), re-packed now unless the batched re-pack of this step already covered it."""
     Cout, Cin = (w.shape[0], w.shape[1] * groups)
     e = _packed_weights(w, plan, mode, groups)
     if not (PACK_BATCHED and e.epoch == _PACK_STATE['epoch'] and e.version == w._version):
         call('tfb_conv3x3_pack_weights', w, e.wp, Cout, Cin, groups, mode, plan['NB'], plan['KC'], plan['c_step'], plan['nchunks'],
              plan['nb_real'], plan['gblocks'])
+    return e
+
+
+def _conv_tc_run(x16, w, bias, plan, mode, c_write, groups, relu, stride=1, want_stats=False):
+    N, H, W, c_read = x16.shape
+    e = _packed_current(w, plan, mode, groups)
     y = torch.empty((N, (H - 1) // stride + 1, (W - 1) // stride + 1, c_write), dtype=torch.float32, device=x16.device)
     st = None
     if want_stats and bias is None and not relu and c_write % 4 == 0 and plan['nb_real'] % 4 == 0:
@@ -888,6 +894,60 @@ def conv2d(x, w, bias=None, stride=1, groups=1, relu=False, bn_stats=False):
     if G.MODE == 'bf16' and w.shape[2] == 3 and stride == 1 and _conv_tc_plan(w.shape[1] * groups, w.shape[0], groups) is not None:
         return Conv3x3TCFn.apply(x, w, bias, groups, relu, bn_stats, implicit)
     return Conv2dFn.apply(x, w, bias, stride, groups, relu, bn_stats, implicit)
+
+
+# ------------------------------------------------------------------ eval-mode BatchNorm in the conv / GEMM epilogue
+def bn_epilogue_path(x, w, stride, groups, residual):
+    """Which tensor-core launch computes bn(conv(x)) of an eval-mode BatchNorm in its epilogue: 'gemm' (1x1 convs, after the
+    stride-2 subsample), 'conv3' (3x3 convs, stride 1 or 2) or None (the conv and batch_norm run as two launches). It follows
+    conv2d's choice of kernel in bf16 mode, so the fused launch has the plain launch's tile plan and gives its bits."""
+    if G.MODE != 'bf16' or x.dim() != 4 or w.shape[0] % 4 != 0:
+        return None
+    if torch.is_grad_enabled() and (x.requires_grad or w.requires_grad):
+        return None                                   # (batch_norm refuses it: eval-mode BatchNorm has no backward)
+    if residual is not None and not BN_ADD_FUSED:
+        return None
+    N, H, W, Cin = x.shape
+    ks, Cout = w.shape[2], w.shape[0]
+    if ks == 1 and groups == 1 and stride in (1, 2):
+        Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+        return 'gemm' if G.tc_ok(N * Ho * Wo, Cout, Cin, Cin, Cout) else None
+    if ks == 3 and (stride == 1 or (stride == 2 and CONV_S2_TC)) and _conv_tc_plan(Cin, Cout, groups) is not None:
+        return 'conv3'
+    return None
+
+
+def conv_bn_eval(x, w, bn, stride=1, groups=1, relu=False, residual=None, emit16=False):
+    """relu?(bn(conv(x)) + residual) of an eval-mode BatchNorm (running statistics) as ONE tensor-core launch whose epilogue
+    normalises, adds the residual, applies the ReLU and writes the fp32 result (and its bf16 sidecar when emit16): the same bits as
+    conv2d + batch_norm, without the unnormalised conv output in memory. None when bn_epilogue_path finds no such launch."""
+    path = bn_epilogue_path(x, w, stride, groups, residual)
+    if path is None:
+        return None
+    invstd = torch.rsqrt(bn.running_var + bn.eps)
+    res = _c(residual) if residual is not None else None
+    Cout = w.shape[0]
+    if path == 'gemm':
+        if stride == 2:
+            x = Subsample2Fn.apply(x)
+        N, H, W, C = x.shape
+        xs = _as16(_c(_view16(x, x.reshape(-1, C))))
+        wb = G.weight_bf16(w.view(Cout, -1))
+        y = torch.empty((N, H, W, Cout), dtype=torch.float32, device=x.device)
+        y16 = _emit16(y, emit16)
+        call('tfb_gemm_bf16_tc_bn_eval', N * H * W, Cout, C, xs, xs.stride(0), wb, wb.stride(0), y, Cout, bn.running_mean, invstd, bn.weight,
+             bn.bias, res, int(relu), y16)
+        return _attach16(y, y16)
+    x = _c(x)
+    N, H, W, Cin = x.shape
+    plan = _conv_tc_plan(Cin, Cout, groups)
+    x16 = _as16(x)
+    e = _packed_current(w, plan, 0, groups)
+    y = torch.empty((N, (H - 1) // stride + 1, (W - 1) // stride + 1, Cout), dtype=torch.float32, device=x.device)
+    y16 = _emit16(y, emit16)
+    call('tfb_conv3x3_tc_bn_eval', x16, e.wp, y, N, H, W, Cin, Cout, plan['NB'], plan['KC'], plan['c_step'], plan['nchunks'], plan['nb_real'],
+         plan['gblocks'], stride, bn.running_mean, invstd, bn.weight, bn.bias, res, int(relu), y16)
+    return _attach16(y, y16)
 
 
 # ------------------------------------------------------------------ normalisation

@@ -2,7 +2,8 @@
 gradient all-reduce, fused AdamW — as a reusable object, optionally captured into ONE CUDA graph and replayed.
 
 This is the body of the reference's `Engine.train()` loop (train.py:304-316) with the synchronising `.item()` calls moved
-out of the step; bench.py and the tests drive it."""
+out of the step; bench.py and the tests drive it. `Validator` is the reference's `Engine.validate()` / `log_losses`
+(train.py:321-379): the eval-mode forward and its loss bookkeeping, also as one CUDA graph."""
 import torch
 import torch.distributed as dist
 
@@ -88,7 +89,8 @@ class Trainer:
                 return loss
         return self._step(d)
 
-    def _step(self, d):
+    def expand_inputs(self, d):
+        """(model inputs, LiDAR BEV) from a batch of `input_keys`: the GPU input pipeline on raw batches, the BEV histogram else."""
         if self.raw_inputs:
             # crop + CHW / normalise, depth decode, class LUT, align + BEV histogram, target-point map: three launches on the raw batch
             raw = dict(rgb=d['rgb_u8'], depth=d['depth_u8'], seg=d['seg_u8'], crop_shift=d['crop_shift'], points=d['points'],
@@ -104,12 +106,14 @@ class Trainer:
             lidar = p['lidar']
         else:
             lidar = bev.lidar_to_histogram_features_batched(d['points'])
+        return d, lidar
+
+    def _step(self, d):
+        d, lidar = self.expand_inputs(d)
         self.opt.zero_grad()
         if self.reducer.pipeline:
             self.opt.begin_step()        # AdamW spans are launched from the backward pass (optim.FusedAdamW.step_span)
-        losses = self.net(d['rgb'], lidar, ego_waypoint=d['ego_waypoint'], target_point=d['target_point'],
-                          target_point_image=d['target_point_image'], ego_vel=d['ego_vel'], bev=d['bev'], label=d['label'],
-                          depth=d['depth'], semantic=d['semantic'], bev_points=d.get('bev_points'), cam_points=d.get('cam_points'))
+        losses = self.forward_losses(d, lidar)
         self.last_losses = losses          # the 11 scalars of this step (device tensors; static buffers under graph replay)
         loss = None
         for k, v in losses.items():
@@ -119,6 +123,12 @@ class Trainer:
         if not self.reducer.replanned and self.graph is None and not torch.cuda.is_current_stream_capturing():
             self.reducer.replan()       # once, after the first backward pass showed the order in which gradients complete
         return loss
+
+    def forward_losses(self, d, lidar):
+        """The model's 11 losses (dict in the model's order) on the expanded inputs."""
+        return self.net(d['rgb'], lidar, ego_waypoint=d['ego_waypoint'], target_point=d['target_point'],
+                        target_point_image=d['target_point_image'], ego_vel=d['ego_vel'], bev=d['bev'], label=d['label'],
+                        depth=d['depth'], semantic=d['semantic'], bev_points=d.get('bev_points'), cam_points=d.get('cam_points'))
 
     def capture(self, example):
         """Captures step() into a CUDA graph over static input buffers shaped like `example` (host or device tensors).
@@ -161,3 +171,115 @@ class Trainer:
         self.graph.replay()
         ops.invalidate_packs()        # the replayed optimizer kernel changed the weights behind Python's back
         return self.static_loss
+
+
+def average_over_ranks(means):
+    """The per-rank means (CPU fp64 tensor) averaged over the ranks of the process group, as log_losses averages the gathered rank
+    means (train.py:344-379): a SUM all-reduce divided by the world size. Without a process group (or with one rank) the means."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
+        return means
+    world = dist.get_world_size()
+    t = means.to('cuda') if dist.get_backend() == 'nccl' else means.clone()
+    dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    return t.cpu() / world
+
+
+class Validator:
+    """Validation of a Trainer's network: the eval-mode forward and the 11 losses of each batch, accumulated on the device as
+    Engine.validate does (train.py:321-342) by tfb_val_accumulate, so a batch needs no host read-back; finish() reads the sums once.
+
+        val = Validator(tr); val.capture(example)
+        for batch in loader: val.load(batch); val.replay()      # (a batch of another size: val.step(batch))
+        means = val.finish()                                    # {'loss_total', 'loss_wp', ...}, averaged over ranks; resets
+
+    It shares the trainer's network, loss weights, input mode and input pipeline, and touches no training state: no tick(), no
+    dropout seed, no running statistics, no optimizer."""
+
+    def __init__(self, trainer):
+        self.tr = trainer
+        self.device = trainer.device
+        self.acc = None
+        self.order = None                  # the model's loss-dict order, fixed by the first forward
+        self.graph = None
+        self.static = None
+        self.graph_launches = 0
+
+    def _losses(self, d):
+        """The eval-mode forward of batch d (input_keys) under no_grad: the packed conv weights are refreshed first by ONE batched
+        re-pack launch (the weights may have changed since the last validation), then the model's losses."""
+        net = self.tr.net
+        was = net.training
+        net.eval()
+        try:
+            with torch.no_grad():
+                ops._prepack_all(self.device)
+                d, lidar = self.tr.expand_inputs(d)
+                return self.tr.forward_losses(d, lidar)
+        finally:
+            net.train(was)
+
+    def _accumulate(self, losses, table):
+        if self.order is None:
+            self.order = list(losses)
+            self.w32 = torch.tensor([self.tr.weights[k] for k in self.order], dtype=torch.float32, device=self.device)
+            self.acc = torch.zeros(len(self.order) + 2, dtype=torch.float64, device=self.device)
+        if list(losses) != self.order:
+            raise RuntimeError('the model returned its losses in another order')
+        if table is None:
+            table = torch.tensor([losses[k].data_ptr() for k in self.order], dtype=torch.int64).to(self.device)
+        _lib.call('tfb_val_accumulate', table, self.w32, len(self.order), self.acc)
+
+    def step(self, batch):
+        """One validation batch, eagerly (any batch size); batch tensors on the host or the device."""
+        d = {k: batch[k].to(self.device, non_blocking=True) for k in self.tr.input_keys}
+        losses = self._losses(d)
+        self._accumulate(losses, None)
+        return losses
+
+    def capture(self, example):
+        """Captures one validation batch (re-pack, eval forward, losses, accumulation) as ONE CUDA graph over static input buffers
+        shaped like `example`. The sums it accumulates during the warm-up are cleared."""
+        self.static = {k: torch.empty(example[k].shape, dtype=example[k].dtype, device=self.device) for k in self.tr.input_keys}
+        self.load(example)
+        side = torch.cuda.Stream(self.device)
+        side.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(side):
+            for _ in range(2):             # registers every packed weight and the batched re-pack table, loads the modules
+                self.step(self.static)
+        torch.cuda.current_stream(self.device).wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        table = torch.empty(len(self.order), dtype=torch.int64, device=self.device)
+        g = torch.cuda.CUDAGraph()
+        l0 = _lib.lib().launches
+        with torch.cuda.graph(g):
+            self.static_losses = self._losses(self.static)
+            self._accumulate(self.static_losses, table)
+        self.graph, self.graph_launches = g, _lib.lib().launches - l0
+        # the graph's losses live at fixed addresses: the table the captured accumulation reads is written once, after the capture
+        table.copy_(torch.tensor([self.static_losses[k].data_ptr() for k in self.order], dtype=torch.int64))
+        self._table = table
+        self.acc.zero_()
+        torch.cuda.synchronize(self.device)
+        return True
+
+    def load(self, batch):
+        for k in self.tr.input_keys:
+            self.static[k].copy_(batch[k], non_blocking=True)
+
+    def replay(self):
+        self.graph.replay()
+        return self.static_losses
+
+    def finish(self):
+        """{'loss_total', 'loss_<name>', ...}: the per-batch means of the validation so far, averaged over the ranks, as log_losses
+        logs them. Resets the sums."""
+        if self.acc is None:
+            raise RuntimeError('no validation batch was run')
+        a = self.acc.cpu()
+        n = len(self.order)
+        if a[n + 1] == 0:
+            raise RuntimeError('no validation batch was run')
+        means = torch.cat([a[n:n + 1], a[:n]]) / a[n + 1]
+        means = average_over_ranks(means)
+        self.acc.zero_()
+        return dict(zip(['loss_total'] + self.order, means.tolist()))
