@@ -472,8 +472,6 @@ class LateFusionBackbone(nn.Module):
         self.config = config
         if config.use_point_pillars:
             raise RuntimeError('PointPillars LiDAR encoder is out of scope (config.py:42 default False)')
-        if use_velocity:
-            raise RuntimeError('use_velocity=True is not implemented (train.py:54 default is 0)')
         in_channels = 2 * config.lidar_seq_len + (1 if config.use_target_point_image else 0)
         check_trunk_pair(image_architecture, lidar_architecture)
         self.image_encoder = _PlainEncoder(image_architecture, 'features', 3, normalize=True)
@@ -481,6 +479,8 @@ class LateFusionBackbone(nn.Module):
         self.norm_after_pool_img = nn.Sequential()
         self.norm_after_pool_lidar = nn.Sequential()
         self.use_velocity = use_velocity
+        if use_velocity:
+            self.vel_emb = nn.Linear(1, config.perception_output_features)     # late_fusion.py:36-39, same registration position
         channel, c_out = config.bev_features_chanels, config.perception_output_features
         # both parameterless when the IMAGE trunk already ends at perception_output_features (late_fusion.py:45-52: "ResNet
         # models were trained without this"); forward skips them then
@@ -497,7 +497,10 @@ class LateFusionBackbone(nn.Module):
             object.__setattr__(self, '_bn_cache', [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)])
         return self._bn_cache
 
-    def forward_nhwc(self, image, lidar):
+    def forward_nhwc(self, image, lidar, velocity=None):
+        """velocity [B, 1]: the ego speed, read with use_velocity (its embedding is added to the fused vector, late_fusion.py:107-109)."""
+        if self.use_velocity and velocity is None:
+            raise RuntimeError('LateFusionBackbone(use_velocity=True) needs the velocity input')
         if self.training:
             torch._foreach_add_([m.num_batches_tracked for m in self._bn_modules()], 1)
             ops.tick(image.device)
@@ -516,6 +519,8 @@ class LateFusionBackbone(nn.Module):
             l = self.lidar_encoder.run(ops.nchw_to_nhwc(lidar))
         x, l = _conv1x1_or_skip(self.reduce_channels_conv_image, x), _conv1x1_or_skip(self.reduce_channels_conv_lidar, l)
         fused = ops.add(ops.PoolHWFn.apply(x), ops.PoolHWFn.apply(l))
+        if self.use_velocity:
+            fused = ops.vel_emb_add(velocity, self.vel_emb, fused)
         f = self.config.bev_upsample_factor
         up = lambda t: ops.upsample(t, t.shape[1] * f, t.shape[2] * f, False, emit16=True)
         p5 = ops.conv2d(l, self.c5_conv.weight, self.c5_conv.bias, relu=True)
@@ -525,7 +530,7 @@ class LateFusionBackbone(nn.Module):
         return (p2, p3, p4, p5), x, fused
 
     def forward(self, image, lidar, velocity):
-        feats, grid, fused = self.forward_nhwc(image, lidar)
+        feats, grid, fused = self.forward_nhwc(image, lidar, velocity)
         return tuple(ops.nhwc_to_nchw(f) for f in feats), ops.nhwc_to_nchw(grid), fused
 
 
@@ -555,11 +560,13 @@ class GeometricFusionBackbone(nn.Module):
     the 4 trunk scales, features of one modality are pooled to its anchor grid, gathered at 5 projected correspondences per
     cell of the other modality's grid, summed, passed through a 3-layer MLP and added back at full resolution.
 
-    Same parameter names / shapes as the reference. Two exact-in-real-arithmetic reassociations keep the work on the
-    anchor grids instead of the full maps (both ops are linear, bilinear weights sum to 1):
+    Same parameter names / shapes as the reference. Three exact-in-real-arithmetic reassociations keep the work on the
+    anchor grids instead of the full maps (the ops are linear, bilinear weights sum to 1):
       avgpool(conv1x1(x))           -> conv1x1(avgpool(x))          (geometric_fusion.py:132-135)
       conv1x1(interpolate(enc))     -> interpolate(conv1x1(enc))    (geometric_fusion.py:150-151)
-    so the 512-channel embeddings only ever exist as [B,5,22,512] / [B,8,8,512]. fp32 rounding differs at the 1e-6 level.
+      (x + interpolate(d)) + e      -> x + interpolate(d + e)       (use_velocity: e = vel_emb_i(v), geometric_fusion.py:142-157)
+    so the 512-channel embeddings only ever exist as [B,5,22,512] / [B,8,8,512], and the speed embedding is added to the
+    [B,8,8,C_i] / [B,5,22,C_i] deconv outputs instead of the full maps. fp32 rounding differs at the 1e-6 level.
     The scale-4 image branch gathers from the scale-3 LiDAR embedding, as the reference does (geometric_fusion.py:277)."""
 
     def __init__(self, config, image_architecture='resnet34', lidar_architecture='resnet18', use_velocity=0):
@@ -567,8 +574,6 @@ class GeometricFusionBackbone(nn.Module):
         self.config = config
         if config.use_point_pillars:
             raise RuntimeError('PointPillars LiDAR encoder is out of scope (config.py:42 default False)')
-        if use_velocity:
-            raise RuntimeError('use_velocity=True is not implemented (train.py:54 default is 0)')
         if config.n_scale != 4:
             raise RuntimeError('n_scale=%r is not implemented (config.py default 4)' % (config.n_scale,))
         self.use_velocity = use_velocity
@@ -577,8 +582,12 @@ class GeometricFusionBackbone(nn.Module):
         self.image_encoder = ImageCNN(architecture=image_architecture, normalize=True)
         self.lidar_encoder = _GeoLidarEncoder(architecture=lidar_architecture, in_channels=in_channels)
         widths, hid = REGNETY_032['widths'], config.n_embd
-        for stem in ('image_conv', 'image_deconv', 'lidar_conv', 'lidar_deconv'):
+        for stem in ('image_conv', 'image_deconv', 'vel_emb', 'lidar_conv', 'lidar_deconv'):
             for i in range(4):
+                if stem == 'vel_emb':
+                    if use_velocity:           # geometric_fusion.py:40-44, registered between image_deconv4 and lidar_conv1
+                        setattr(self, 'vel_emb%d' % (i + 1), nn.Linear(1, widths[i]))
+                    continue
                 cin, cout = (hid, widths[i]) if 'deconv' in stem else (widths[i], hid)
                 setattr(self, '%s%d' % (stem, i + 1), nn.Conv2d(cin, cout, 1))
         for stem in ('image_projection', 'lidar_projection'):
@@ -604,11 +613,14 @@ class GeometricFusionBackbone(nn.Module):
             x = ops.linear(x, mlp[j].weight, mlp[j].bias, relu=True)
         return x
 
-    def forward_nhwc(self, image, lidar, bev_points, img_points):
+    def forward_nhwc(self, image, lidar, bev_points, img_points, velocity=None):
         """image NCHW 0..255, lidar NCHW, bev_points [B,8,8,5,2] / img_points int64 (x, y) correspondences. img_points is read
         flat as [B, 5, 22, 5, 2] whatever its shape, as the reference's .view does (geometric_fusion.py:147): the [B,22,5,5,2] the
-        reference's dataset makes (x-major camera cells, data.py:637) is reinterpreted as (h, w) = (5, 22) row-major."""
+        reference's dataset makes (x-major camera cells, data.py:637) is reinterpreted as (h, w) = (5, 22) row-major.
+        velocity [B, 1]: the ego speed, read with use_velocity."""
         cfg = self.config
+        if self.use_velocity and velocity is None:
+            raise RuntimeError('GeometricFusionBackbone(use_velocity=True) needs the velocity input')
         if self.training:
             torch._foreach_add_([m.num_batches_tracked for m in self._bn_modules()], 1)
             ops.tick(image.device)
@@ -632,6 +644,9 @@ class GeometricFusionBackbone(nn.Module):
             ld, idc = getattr(self, 'lidar_deconv%d' % i), getattr(self, 'image_deconv%d' % i)
             dl = ops.linear(bev_enc, ld.weight, ld.bias)                                    # [B,8,8,C_i]
             dx = ops.linear(img_enc, idc.weight, idc.bias)                                  # [B,5,22,C_i]
+            if self.use_velocity:
+                # geometric_fusion.py:142-271: vel_emb_i(v) added to both maps of the scale, here on the anchor grids
+                dl, dx = ops.vel_emb_add(velocity, getattr(self, 'vel_emb%d' % i), dl, dx)
             if i < 4:
                 dl = ops.upsample(dl, l.shape[1], l.shape[2], False)
                 dx = ops.upsample(dx, x.shape[1], x.shape[2], False)
@@ -650,7 +665,7 @@ class GeometricFusionBackbone(nn.Module):
         return (p2, p3, p4, p5), x, fused
 
     def forward(self, image, lidar, velocity, bev_points, img_points):
-        feats, grid, fused = self.forward_nhwc(image, lidar, bev_points, img_points)
+        feats, grid, fused = self.forward_nhwc(image, lidar, bev_points, img_points, velocity)
         return tuple(ops.nhwc_to_nchw(f) for f in feats), ops.nhwc_to_nchw(grid), fused
 
 

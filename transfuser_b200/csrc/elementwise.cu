@@ -679,6 +679,60 @@ __global__ void __launch_bounds__(256) bcast_add_nc_kernel(const float* __restri
     y[i] = x[i] + v[(i / tc) * C + i % C];
 }
 
+// y_k[b][t][c] = x_k[b][t][c] + fmaf(v[b], w[c], bias[c]) for one or two tensors x_k [B, T_k, C]: one CTA per (k, b, t) row, the
+// threads stride over the channels.
+__global__ void __launch_bounds__(128) vel_emb_add_kernel(const float* __restrict__ v, const float* __restrict__ w,
+                                                          const float* __restrict__ bias, const float* __restrict__ x0,
+                                                          float* __restrict__ y0, int T0, const float* __restrict__ x1,
+                                                          float* __restrict__ y1, int T1, int B, int C) {
+  int row = blockIdx.x;
+  const float* x = x0;
+  float* y = y0;
+  int T = T0;
+  if (row >= B * T0) { row -= B * T0; x = x1; y = y1; T = T1; }
+  const float vb = v[row / T];
+  const int64_t off = (int64_t)row * C;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) y[off + c] = x[off + c] + fmaf(vb, w[c], bias[c]);
+}
+
+// dbias[c] = sum_b s_b[c], dw[c] = sum_b v[b] s_b[c], s_b[c] = sum_k sum_t dy_k[b][t][c]. One CTA owns VEB_CW channels whole: no
+// cross-CTA fold, no atomics. Thread row ty sums t = ty, ty + VEB_TR, ... in increasing t; the VEB_TR row partials are folded in
+// ty order; then k, then b in increasing order (the exact order is spelled out at tfb_vel_emb_bwd).
+constexpr int VEB_CW = 32, VEB_TR = 16;
+__global__ void __launch_bounds__(VEB_CW * VEB_TR) vel_emb_bwd_kernel(const float* __restrict__ v, const float* __restrict__ dy0, int T0,
+                                                                      const float* __restrict__ dy1, int T1, int B, int C,
+                                                                      float* __restrict__ dw, float* __restrict__ dbias) {
+  __shared__ float part[2][VEB_TR][VEB_CW];
+  const int tx = threadIdx.x, ty = threadIdx.y, c = blockIdx.x * VEB_CW + tx;
+  const bool live = c < C;
+  float acc_b = 0.f, acc_w = 0.f;
+  for (int b = 0; b < B; ++b) {
+    float p0 = 0.f, p1 = 0.f;
+    if (live) {
+      const float* d0 = dy0 + (int64_t)b * T0 * C + c;
+#pragma unroll 4
+      for (int t = ty; t < T0; t += VEB_TR) p0 += d0[(int64_t)t * C];
+      if (dy1) {
+        const float* d1 = dy1 + (int64_t)b * T1 * C + c;
+#pragma unroll 4
+        for (int t = ty; t < T1; t += VEB_TR) p1 += d1[(int64_t)t * C];
+      }
+    }
+    part[0][ty][tx] = p0;
+    part[1][ty][tx] = p1;
+    __syncthreads();
+    if (ty == 0) {
+      float s0 = 0.f, s1 = 0.f;
+      for (int r = 0; r < VEB_TR; ++r) { s0 += part[0][r][tx]; s1 += part[1][r][tx]; }
+      const float s = dy1 ? s0 + s1 : s0;
+      acc_b += s;
+      acc_w = fmaf(v[b], s, acc_w);
+    }
+    __syncthreads();
+  }
+  if (ty == 0 && live) { dbias[c] = acc_b; dw[c] = acc_w; }
+}
+
 // y = x * (*s) * k  (device-resident scalar: no host sync)  /  y += ...
 __global__ void __launch_bounds__(256) scale_dev_kernel(const float* __restrict__ x, const float* __restrict__ s, float k,
                                                         float* __restrict__ y, int64_t n, int accumulate) {
@@ -1087,6 +1141,36 @@ TFB_API int tfb_bcast_add_nc(const float* x, const float* v, float* y, int N, in
   TFB_REQUIRE(x && v && y && N > 0 && T > 0 && C > 0);
   const int64_t total = (int64_t)N * T * C;
   bcast_add_nc_kernel<<<tfb_grid(total, 256), 256, 0, stream>>>(x, v, y, total, T, C);
+  TFB_CHECK_LAUNCH();
+  return TFB_OK;
+}
+// The ego-speed embedding Linear(1, C) added to one or two feature tensors (reference late_fusion.py:107-109: the fused vector;
+// geometric_fusion.py:142-271: the LiDAR and the image map of one scale). v [B] speeds, w [C] (the [C, 1] weight), bias [C];
+// x0 / y0 [B, T0, C] and optionally x1 / y1 [B, T1, C] (x1 = y1 = null, T1 = 0 for one tensor).
+//   y_k[b, t, c] = x_k[b, t, c] + e[b, c],   e[b, c] = fmaf(v[b], w[c], bias[c])   (__fmaf_rn: one rounding; then one fp32 add)
+// No e tensor is formed.
+TFB_API int tfb_vel_emb_add(const float* v, const float* w, const float* bias, const float* x0, float* y0, int T0, const float* x1, float* y1,
+                            int T1, int B, int C, cudaStream_t stream) {
+  TFB_REQUIRE(v && w && bias && x0 && y0 && T0 > 0 && B > 0 && C > 0 && T1 >= 0);
+  TFB_REQUIRE(T1 == 0 ? (!x1 && !y1) : (x1 && y1));
+  const int64_t rows = (int64_t)B * (T0 + T1);
+  TFB_REQUIRE(rows <= 0x7fffffffLL);
+  vel_emb_add_kernel<<<(unsigned)rows, 128, 0, stream>>>(v, w, bias, x0, y0, T0, x1, y1, T1, B, C);
+  TFB_CHECK_LAUNCH();
+  return TFB_OK;
+}
+// Backward of tfb_vel_emb_add for the embedding's parameters (dx_k = dy_k needs no kernel): dw [C] (the [C, 1] weight's gradient)
+// and dbias [C], both overwritten. Deterministic fixed-order fp32 sums, for every channel c:
+//   p_k[r]  = sum over t = r, r + 16, r + 32, ... < T_k of dy_k[b, t, c], in increasing t            (r = 0 .. 15)
+//   S_k     = sum over r = 0 .. 15 of p_k[r], in increasing r
+//   s_b     = S_0 + S_1   (S_0 alone with one tensor)
+//   dbias   = sum over b of s_b, in increasing b;   dw = fmaf(v[b], s_b, dw) over increasing b, from 0
+// every sum starting from 0.f. One CTA per 32 channels; no atomics, the same bits on every run.
+TFB_API int tfb_vel_emb_bwd(const float* v, const float* dy0, int T0, const float* dy1, int T1, int B, int C, float* dw, float* dbias,
+                            cudaStream_t stream) {
+  TFB_REQUIRE(v && dy0 && dw && dbias && T0 > 0 && B > 0 && C > 0 && T1 >= 0);
+  TFB_REQUIRE(T1 == 0 ? !dy1 : dy1 != nullptr);
+  vel_emb_bwd_kernel<<<(C + VEB_CW - 1) / VEB_CW, dim3(VEB_CW, VEB_TR), 0, stream>>>(v, dy0, T0, dy1, T1, B, C, dw, dbias);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }

@@ -145,14 +145,18 @@ class LidarCenterNet(nn.Module):
                                   self.pred_len, float(self.config.lidar_pos[0]))
         return pred_wp, None, None, None, None
 
+    def _uses_velocity(self):
+        m = self._model
+        return bool(m.transformer1.use_velocity if self.backbone in ('transFuser', 'latentTF') else m.use_velocity)
+
     def _run_backbone(self, rgb, lidar_bev, bev_points, cam_points, ego_vel=None):
+        # model.py:753 passes ego_vel [B, 1] to every backbone; only one built with use_velocity reads it
+        vel = ego_vel if self._uses_velocity() else None
         if self.backbone == 'geometric_fusion':
             if bev_points is None or cam_points is None:
                 raise RuntimeError('the geometric_fusion backbone needs bev_points and cam_points (train.py:281-288)')
-            return self._model.forward_nhwc(rgb, lidar_bev, bev_points, cam_points)
-        if self.backbone in ('transFuser', 'latentTF') and self._model.transformer1.use_velocity:   # (latentTF.py:144-195: same GPTs)
-            return self._model.forward_nhwc(rgb, lidar_bev, velocity=ego_vel)      # model.py:753 passes ego_vel to the backbone
-        return self._model.forward_nhwc(rgb, lidar_bev)
+            return self._model.forward_nhwc(rgb, lidar_bev, bev_points, cam_points, velocity=vel)
+        return self._model.forward_nhwc(rgb, lidar_bev, velocity=vel)
 
     def get_bbox_local_metric(self, bbox):
         """model.py:810-842: one decoded row (x, y, w, h, yaw, speed, brake, confidence; LiDAR-BEV pixels) -> (6x3 array: the

@@ -1312,6 +1312,46 @@ class BcastAddTokensFn(Function):
         return dy, dv
 
 
+class VelEmbAddFn(Function):
+    """x_k + vel_emb(v) for every token / pixel of each x_k [B, ..., C] (one or two tensors): the ego-speed embedding Linear(1, C)
+    computed inside tfb_vel_emb_add, no [B, C] embedding tensor. One node per embedding, so its weight and bias gradients are
+    written once per step, straight into the flat gradient buffer (tfb_vel_emb_bwd). The speed is an input: it gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, velocity, weight, bias, *xs):
+        B, C = xs[0].shape[0], xs[0].shape[-1]
+        if len(xs) not in (1, 2) or any(x.shape[0] != B or x.shape[-1] != C for x in xs):
+            raise ValueError('VelEmbAddFn takes one or two tensors [B, ..., C] of one batch and width')
+        if velocity.numel() != B or tuple(weight.shape) != (C, 1) or tuple(bias.shape) != (C,):
+            raise ValueError('VelEmbAddFn: the speed must be [B, 1] and the embedding Linear(1, %d)' % C)
+        v = _c(velocity.reshape(B).to(torch.float32))
+        xs = [_c(x) for x in xs]
+        ys = [torch.empty_like(x) for x in xs]
+        T = [x.numel() // (B * C) for x in xs]
+        x1, y1, T1 = (xs[1], ys[1], T[1]) if len(xs) == 2 else (None, None, 0)
+        call('tfb_vel_emb_add', v, weight, bias, xs[0], ys[0], T[0], x1, y1, T1, B, C)
+        ctx.save_for_backward(v, weight, bias)
+        ctx.T = T
+        return ys[0] if len(ys) == 1 else tuple(ys)
+
+    @staticmethod
+    def backward(ctx, *dys):
+        v, weight, bias = ctx.saved_tensors
+        if ctx.needs_input_grad[0]:
+            raise RuntimeError('VelEmbAddFn does not differentiate with respect to the speed input')
+        dys = [_c(d) for d in dys]
+        B, C = dys[0].shape[0], dys[0].shape[-1]
+        dw, db = _gbuf(weight), _gbuf(bias)
+        d1, T1 = (dys[1], ctx.T[1]) if len(dys) == 2 else (None, 0)
+        call('tfb_vel_emb_bwd', v, dys[0], ctx.T[0], d1, T1, B, C, dw, db)
+        return (None, dw, db) + tuple(dys)
+
+
+def vel_emb_add(velocity, emb, *xs):
+    """xs with the speed embedding `emb` (an nn.Linear(1, C)) added to every position, as VelEmbAddFn."""
+    return VelEmbAddFn.apply(velocity, emb.weight, emb.bias, *xs)
+
+
 class AddDropoutFn(Function):
     """res + dropout(x) in one pass (the GPT block's residual connections, transfuser.py:546-547); backward regenerates the mask."""
 

@@ -26,7 +26,7 @@ DATASET_KEYS = tuple(k for k in RAW_KEYS if k != 'bev') + ('n_valid', 'bev_u8', 
 
 class Trainer:
     def __init__(self, cfg, device, gemm_mode='bf16', lr=1e-4, seed=0, n_chunks=int(os.environ.get('TFB_GRAD_CHUNKS', '8')), backbone='transFuser',
-                 raw_inputs=False, image_architecture='regnety_032', lidar_architecture='regnety_032'):
+                 raw_inputs=False, image_architecture='regnety_032', lidar_architecture='regnety_032', use_velocity=False):
         self.cfg, self.device = cfg, device
         self.raw_inputs = raw_inputs
         if raw_inputs not in (False, True, 'dataset'):
@@ -42,7 +42,7 @@ class Trainer:
         self.world = dist.get_world_size() if dist.is_initialized() else 1
         gemm.set_mode(gemm_mode)
         ops.manual_seed(1234 + seed)
-        self.net = LidarCenterNet(cfg, device, backbone, image_architecture, lidar_architecture, use_velocity=False).train()
+        self.net = LidarCenterNet(cfg, device, backbone, image_architecture, lidar_architecture, use_velocity=use_velocity).train()
         self.flat = optim.flatten(self.net)
         if self.world > 1:
             # replicas start identical whatever the caller's RNG state: rank 0's parameters and buffers win (DDP does the same at
