@@ -19,6 +19,20 @@ RESNET_DEPTHS = {'resnet18': (2, 2, 2, 2), 'resnet34': (3, 4, 6, 3)}
 RESNET_WIDTHS = (64, 128, 256, 512)
 
 
+def _bn_modules(net):
+    """The BatchNorms of `net` (nn.BatchNorm2d or nn.SyncBatchNorm), one per num_batches_tracked counter: an alias pair such as
+    stem.bn / bn1 is one module, or two modules sharing their tensors after nn.SyncBatchNorm.convert_sync_batchnorm (which keeps the
+    tensors, so a list cached before a conversion still reaches every counter)."""
+    if not hasattr(net, '_bn_cache'):
+        seen, out = set(), []
+        for m in net.modules():
+            if isinstance(m, nn.modules.batchnorm._BatchNorm) and id(m.num_batches_tracked) not in seen:
+                seen.add(id(m.num_batches_tracked))
+                out.append(m)
+        object.__setattr__(net, '_bn_cache', out)
+    return net._bn_cache
+
+
 def _conv_bn(conv, bn, x, stride=1, groups=1, act=True, emit16=False, residual=None, pool=False):
     """bn(conv(x)) with the ReLU (act), the residual add and the SE pool fused into the BatchNorm passes (see _ConvBn.run). An
     eval-mode BatchNorm runs inside the tensor-core conv's epilogue where there is one (ops.conv_bn_eval)."""
@@ -379,9 +393,7 @@ class TransfuserBackbone(nn.Module):
         return LidarEncoder(architecture=architecture, in_channels=in_channels, out_features=self.config.perception_output_features)
 
     def _bn_modules(self):
-        if not hasattr(self, '_bn_cache'):
-            object.__setattr__(self, '_bn_cache', [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)])
-        return self._bn_cache
+        return _bn_modules(self)
 
     def forward_nhwc(self, image, lidar, taps=None, velocity=None):
         """image: NCHW 0..255, lidar: NCHW -> (p2..p5 NHWC), image grid NHWC, fused [B,512]. `taps` (optional dict) receives the
@@ -493,9 +505,7 @@ class LateFusionBackbone(nn.Module):
         self.c5_conv = nn.Conv2d(c_out, channel, (1, 1))
 
     def _bn_modules(self):
-        if not hasattr(self, '_bn_cache'):
-            object.__setattr__(self, '_bn_cache', [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)])
-        return self._bn_cache
+        return _bn_modules(self)
 
     def forward_nhwc(self, image, lidar, velocity=None):
         """velocity [B, 1]: the ego speed, read with use_velocity (its embedding is added to the fused vector, late_fusion.py:107-109)."""
@@ -603,9 +613,7 @@ class GeometricFusionBackbone(nn.Module):
         self.c5_conv = nn.Conv2d(c_out, channel, (1, 1))
 
     def _bn_modules(self):
-        if not hasattr(self, '_bn_cache'):
-            object.__setattr__(self, '_bn_cache', [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)])
-        return self._bn_cache
+        return _bn_modules(self)
 
     @staticmethod
     def _project(mlp, x):

@@ -15,6 +15,7 @@ namespace {
 //   kind 1: BatchNorm forward  -> save_mean, save_invstd, running statistics        (sums = [sum x | sum x^2])
 //   kind 2: BatchNorm backward -> dgamma = sum g*xhat, dbeta = sum g                 (sums = [sum g | sum g*xhat])
 //   kind 3: column sum         -> out[c] = sum                                        (sums = [sum])
+//   kind 4: BatchNorm forward of one rank of a synchronized BatchNorm -> `slice` only, + slice[2C] = M   (sums = [sum x | sum x^2])
 struct Finalize {
   int kind;
   int nsums;             // doubles in use (C or 2C); the counter lives at sums[nsums]
@@ -29,7 +30,27 @@ struct Finalize {
   double* part;          // [nsplit][nsums]: each row split's partial sums; the last block of a slab adds them in split order, so the
                          // result is the same bits on every run (set by the launcher, see alloc_partials)
   unsigned int* cnt;     // one arrival counter per channel slab, in the stream's scratch (alloc_partials)
+  double* slice;         // optional: the folded sums are also written here in fp64 (a rank's slice of a synchronized BatchNorm)
 };
+
+// save_mean / save_invstd / running statistics of channel c from its sums over N rows (N = M, or the count summed over the ranks of a
+// synchronized BatchNorm); returns invstd. Null save_mean / running_mean: not written.
+__device__ __forceinline__ float bn_publish(int c, double s0, double s1, double N, float eps, float momentum, float* __restrict__ save_mean,
+                                            float* __restrict__ save_invstd, float* __restrict__ running_mean, float* __restrict__ running_var,
+                                            double* mean_out = nullptr) {
+  const double mean = s0 / N;
+  double var = s1 / N - mean * mean;
+  if (var < 0.0) var = 0.0;
+  const float invstd = (float)(1.0 / sqrt(var + (double)eps));
+  if (save_mean) { save_mean[c] = (float)mean; save_invstd[c] = invstd; }
+  if (running_mean) {
+    const double unbiased = N > 1.0 ? var * N / (N - 1.0) : var;
+    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)mean;
+    running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unbiased;
+  }
+  if (mean_out) *mean_out = mean;
+  return invstd;
+}
 
 // The partials of channel slab `slab` (channels [slab * slab_w, +slab_w)) come from the nsplit blocks of that slab; the last of them
 // to arrive (arrival counter f.cnt[slab]) folds the slab's channels in split order and finalises them, so the slabs finish in parallel.
@@ -61,21 +82,16 @@ __device__ __forceinline__ void finalize_last_block(double* sums, int C, const F
   for (int i = tid; i < w; i += nthr) {
     const int c = lo + i;
     const double s0 = fs[0][i], s1 = nq > 1 ? fs[1][i] : 0.0;
+    if (f.slice) {
+      f.slice[c] = s0;
+      if (nq > 1) f.slice[C + c] = s1;
+    }
     if (f.kind == 1) {
-      const double mean = s0 / (double)f.M;
-      double var = s1 / (double)f.M - mean * mean;
-      if (var < 0.0) var = 0.0;
-      f.o0[c] = (float)mean;
-      f.o1[c] = (float)(1.0 / sqrt(var + (double)f.eps));
-      if (f.running_mean) {
-        const double unbiased = f.M > 1 ? var * (double)f.M / (double)(f.M - 1) : var;
-        f.running_mean[c] = (1.f - f.momentum) * f.running_mean[c] + f.momentum * (float)mean;
-        f.running_var[c] = (1.f - f.momentum) * f.running_var[c] + f.momentum * (float)unbiased;
-      }
+      bn_publish(c, s0, s1, (double)f.M, f.eps, f.momentum, f.o0, f.o1, f.running_mean, f.running_var);
     } else if (f.kind == 2) {
       f.o0[c] = (float)s0;
       f.o1[c] = (float)s1;
-    } else {
+    } else if (f.kind == 3) {
       f.o0[c] = (float)s0;
     }
     sums[c] = 0.0;
@@ -83,6 +99,7 @@ __device__ __forceinline__ void finalize_last_block(double* sums, int C, const F
   }
   if (slab == 0)
     for (int i = tid; i < f.zero_n; i += nthr) f.zero_buf[i] = 0.f;
+  if (f.kind == 4 && slab == 0 && tid == 0) f.slice[f.nsums] = (double)f.M;
   if (tid == 0) f.cnt[slab] = 0u;    // the stream's scratch counters are zero on entry
 }
 
@@ -371,25 +388,16 @@ __device__ __forceinline__ void bn_params_from_stats(const double* __restrict__ 
                                                      const float* __restrict__ gamma, const float* __restrict__ beta, float* s_scale,
                                                      float* s_shift, bool publish, float* __restrict__ save_mean,
                                                      float* __restrict__ save_invstd, float* __restrict__ running_mean,
-                                                     float* __restrict__ running_var) {
+                                                     float* __restrict__ running_var, const double* __restrict__ count) {
   const int tid = threadIdx.y * blockDim.x + threadIdx.x, nthr = blockDim.x * blockDim.y;
+  const double N = count ? *count : (double)M;      // count: the rows of every rank of a synchronized BatchNorm
   for (int c = tid; c < C; c += nthr) {
-    const double mean = stats[c] / (double)M;
-    double var = stats[C + c] / (double)M - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const float invstd = (float)(1.0 / sqrt(var + (double)eps));
+    double mean;
+    const float invstd = bn_publish(c, stats[c], stats[C + c], N, eps, momentum, publish ? save_mean : nullptr, save_invstd,
+                                    publish ? running_mean : nullptr, running_var, &mean);
     const float sc = gamma[c] * invstd;
     s_scale[c] = sc;
     s_shift[c] = fmaf(-(float)mean, sc, beta[c]);
-    if (publish) {
-      save_mean[c] = (float)mean;
-      save_invstd[c] = invstd;
-      if (running_mean) {
-        const double unbiased = M > 1 ? var * (double)M / (double)(M - 1) : var;
-        running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)mean;
-        running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unbiased;
-      }
-    }
   }
   __syncthreads();
 }
@@ -398,11 +406,13 @@ __global__ void __launch_bounds__(256)
 bn_apply_stats_kernel(const float* __restrict__ x, float* __restrict__ y, int64_t total4, int C, int64_t M, const double* __restrict__ stats,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum, int relu,
                       float* __restrict__ save_mean, float* __restrict__ save_invstd, float* __restrict__ running_mean,
-                      float* __restrict__ running_var, __nv_bfloat16* __restrict__ y16, const float* __restrict__ res) {
+                      float* __restrict__ running_var, __nv_bfloat16* __restrict__ y16, const float* __restrict__ res,
+                      const double* __restrict__ count) {
   __shared__ __align__(16) float s_par[2 * kBnStatsMaxC];
   float* s_scale = s_par;
   float* s_shift = s_par + kBnStatsMaxC;
-  bn_params_from_stats(stats, C, M, eps, momentum, gamma, beta, s_scale, s_shift, blockIdx.x == 0, save_mean, save_invstd, running_mean, running_var);
+  bn_params_from_stats(stats, C, M, eps, momentum, gamma, beta, s_scale, s_shift, blockIdx.x == 0, save_mean, save_invstd, running_mean, running_var,
+                       count);
   const int C4 = C / 4;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % C4) * 4;
@@ -425,12 +435,13 @@ __global__ void __launch_bounds__(256)
 bn_apply_pool_stats_kernel(const float* __restrict__ x, float* __restrict__ y, int HW, int C, int64_t M, const double* __restrict__ stats,
                            const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum, int relu,
                            float* __restrict__ save_mean, float* __restrict__ save_invstd, float* __restrict__ running_mean,
-                           float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw, OrderedSum os) {
+                           float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw, OrderedSum os,
+                           const double* __restrict__ count) {
   __shared__ __align__(16) float s_par[2 * kBnStatsMaxC];
   float* s_scale = s_par;
   float* s_shift = s_par + kBnStatsMaxC;
   bn_params_from_stats(stats, C, M, eps, momentum, gamma, beta, s_scale, s_shift, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0,
-                       save_mean, save_invstd, running_mean, running_var);
+                       save_mean, save_invstd, running_mean, running_var, count);
   __shared__ float4 sm[8][33];
   const int n = blockIdx.y, c = (blockIdx.x * 32 + threadIdx.x) * 4;
   float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -465,12 +476,13 @@ __global__ void __launch_bounds__(256)
 bn_apply_pool_stats_flat_kernel(const float* __restrict__ x, float* __restrict__ y, int HW, int C, int64_t M, const double* __restrict__ stats,
                                 const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum, int relu,
                                 float* __restrict__ save_mean, float* __restrict__ save_invstd, float* __restrict__ running_mean,
-                                float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw, OrderedSum os) {
+                                float* __restrict__ running_var, float* __restrict__ pooled, float inv_hw, OrderedSum os,
+                                const double* __restrict__ count) {
   __shared__ __align__(16) float s_par[2 * 512];
   float* s_scale = s_par;
   float* s_shift = s_par + 512;
   bn_params_from_stats(stats, C, M, eps, momentum, gamma, beta, s_scale, s_shift, blockIdx.x == 0 && blockIdx.y == 0, save_mean, save_invstd,
-                       running_mean, running_var);
+                       running_mean, running_var, count);
   const int C4 = C / 4, RPB = 256 / C4;
   const int t = threadIdx.x, q = t % C4, rr = t / C4, n = blockIdx.y;
   float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -506,11 +518,11 @@ bn_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ dy, f
                     const double* __restrict__ sums, const float* __restrict__ mean, const float* __restrict__ invstd,
                     const float* __restrict__ gamma, const float* __restrict__ beta, int relu, const float* __restrict__ dgamma,
                     const float* __restrict__ dbeta, __nv_bfloat16* __restrict__ dx16, const float* __restrict__ ymask,
-                    float* __restrict__ gout, const float* __restrict__ se_gate = nullptr, const float* __restrict__ se_dpool = nullptr,
-                    int hw = 1) {
+                    float* __restrict__ gout, const float* __restrict__ se_gate, const float* __restrict__ se_dpool, int hw,
+                    const double* __restrict__ count) {
   const int C4 = C / 4;
   const int64_t total4 = M * C4;
-  const double invM = 1.0 / (double)M;
+  const double invM = 1.0 / (count ? *count : (double)M);     // count: the rows of every rank of a synchronized BatchNorm
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % C4) * 4;
     const float4 xv = reinterpret_cast<const float4*>(x)[i];
@@ -720,6 +732,43 @@ template <int MODE>
 int launch_colreduce(const float* x, int64_t ldx, const float* dy, int64_t M, int C, double* out, const float* mean, const float* invstd,
                      const float* gamma, const float* beta, int relu, const float* ymask, Finalize fin, cudaStream_t stream);
 
+// ---- synchronized BatchNorm: the W ranks' slices [W][stride] (gathered in rank order) folded per value in rank order from +0, the
+// rule of ordered_fold, so every rank derives the same bits whatever the collective's algorithm, and one rank gives +0 + s = s.
+//   forward  (stride 2C + 1, [sum x | sum x^2 | count]): folded = the sums over all ranks (count included); save_mean / save_invstd and
+//            the running statistics from them (bn_publish with N = the total count); `zero_buf` cleared (the SE pooling accumulator).
+//   backward (stride 2C, [sum g | sum g*xhat]): gsum = the folded sums rounded to fp32, as tfb_bn_bwd's dbeta / dgamma are.
+__global__ void __launch_bounds__(256)
+bn_sync_fold_kernel(const double* __restrict__ g, int W, int C, int fwd, float eps, float momentum, float* __restrict__ save_mean,
+                    float* __restrict__ save_invstd, float* __restrict__ running_mean, float* __restrict__ running_var,
+                    double* __restrict__ folded, float* __restrict__ gsum, float* __restrict__ zero_buf, int zero_n) {
+  const int stride = fwd ? 2 * C + 1 : 2 * C;
+  const int tid = blockIdx.x * blockDim.x + threadIdx.x, nthr = gridDim.x * blockDim.x;
+  for (int c = tid; c < C; c += nthr) {
+    double s0 = 0.0, s1 = 0.0, n = 0.0;
+    for (int w = 0; w < W; ++w) {
+      const double* sl = g + (int64_t)w * stride;
+      s0 += sl[c];
+      s1 += sl[C + c];
+      if (fwd) n += sl[2 * C];
+    }
+    if (fwd) {
+      folded[c] = s0;
+      folded[C + c] = s1;
+      if (c == 0) folded[2 * C] = n;
+      bn_publish(c, s0, s1, n, eps, momentum, save_mean, save_invstd, running_mean, running_var);
+    } else {
+      gsum[c] = (float)s0;
+      gsum[C + c] = (float)s1;
+    }
+  }
+  for (int i = tid; i < zero_n; i += nthr) zero_buf[i] = 0.f;
+}
+
+// a rank's forward slice from statistics its producer's epilogue accumulated: [stats (2C) | M]
+__global__ void __launch_bounds__(256) bn_sync_slice_copy_kernel(const double* __restrict__ stats, int C, int64_t M, double* __restrict__ slice) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= 2 * C; i += gridDim.x * blockDim.x) slice[i] = i < 2 * C ? stats[i] : (double)M;
+}
+
 // d[n, hw, c] = dy * gate[n][c] + dpool[n][c] * inv_hw  (float4 per thread; C % 4 == 0)
 __global__ void __launch_bounds__(256) scale_gate_kernel(const float* __restrict__ dy, const float* __restrict__ gate,
                                                          const float* __restrict__ dpool, float inv_hw, float* __restrict__ d, int64_t total4,
@@ -792,6 +841,12 @@ int launch_colreduce(const float* x, int64_t ldx, const float* dy, int64_t M, in
 
 }  // namespace
 
+static int bn_apply_launch(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, int relu, const float* save_mean,
+                           const float* save_invstd, void* y16_bf16, const float* residual, float* pooled, int pool_batch, cudaStream_t stream);
+static int bn_apply_stats_launch(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, float eps, float momentum,
+                                 int relu, float* running_mean, float* running_var, float* save_mean, float* save_invstd, const double* stats,
+                                 const double* count, void* y16_bf16, const float* residual, float* pooled, int pool_batch, cudaStream_t stream);
+
 // sums_ws: (2*C + 1) doubles, ZERO on entry, left zero on exit (shared by all layers of a stream; no memset launches).
 // y16_bf16 (optional): bf16 copy of y written in the same pass (operand of the next layer's tensor-core GEMM / conv).
 // residual (optional, [M, C]): y = act(bn(x) + residual) — the Bottleneck's last BatchNorm + shortcut add + ReLU in one pass.
@@ -806,6 +861,12 @@ TFB_API int tfb_bn_fwd(const float* x, float* y, int64_t M, int C, const float* 
   Finalize fin = {1, 2 * C, M, eps, momentum, save_mean, save_invstd, running_mean, running_var, pooled, pooled ? pool_batch * C : 0};
   const int rc = launch_colreduce<0>(x, C, nullptr, M, C, sums_ws, nullptr, nullptr, nullptr, nullptr, 0, nullptr, fin, stream);
   if (rc != TFB_OK) return rc;
+  return bn_apply_launch(x, y, M, C, gamma, beta, relu, save_mean, save_invstd, y16_bf16, residual, pooled, pool_batch, stream);
+}
+
+// The normalise pass of tfb_bn_fwd from save_mean / save_invstd; `pooled` zero on entry.
+static int bn_apply_launch(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, int relu, const float* save_mean,
+                           const float* save_invstd, void* y16_bf16, const float* residual, float* pooled, int pool_batch, cudaStream_t stream) {
   if (pooled) {
     const int HW = (int)(M / pool_batch);
     int splits = (HW + 255) / 256;
@@ -833,6 +894,14 @@ TFB_API int tfb_bn_fwd_stats(const float* x, float* y, int64_t M, int C, const f
                              void* y16_bf16, const float* residual, float* pooled, int pool_batch, cudaStream_t stream) {
   TFB_REQUIRE(x && y && gamma && beta && save_mean && save_invstd && stats && M > 0 && C > 0 && C % 4 == 0 && C <= kBnStatsMaxC);
   TFB_REQUIRE(!pooled || (pool_batch > 0 && M % pool_batch == 0 && !y16_bf16 && !residual));
+  return bn_apply_stats_launch(x, y, M, C, gamma, beta, eps, momentum, relu, running_mean, running_var, save_mean, save_invstd, stats, nullptr,
+                               y16_bf16, residual, pooled, pool_batch, stream);
+}
+
+// The body of tfb_bn_fwd_stats; count (optional, device): the row count the statistics were summed over, in place of M.
+static int bn_apply_stats_launch(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, float eps, float momentum,
+                                 int relu, float* running_mean, float* running_var, float* save_mean, float* save_invstd, const double* stats,
+                                 const double* count, void* y16_bf16, const float* residual, float* pooled, int pool_batch, cudaStream_t stream) {
   if (pooled) {
     const int HW = (int)(M / pool_batch);
     int splits = (HW + 255) / 256;
@@ -847,7 +916,8 @@ TFB_API int tfb_bn_fwd_stats(const float* x, float* y, int64_t M, int C, const f
       const int rc = ordered_alloc(os, sp, (int64_t)pool_batch * C, stream);
       if (rc != TFB_OK) return rc;
       bn_apply_pool_stats_flat_kernel<<<dim3(sp, pool_batch), 256, 0, stream>>>(x, y, HW, C, M, stats, gamma, beta, eps, momentum, relu, save_mean,
-                                                                               save_invstd, running_mean, running_var, pooled, 1.f / (float)HW, os);
+                                                                               save_invstd, running_mean, running_var, pooled, 1.f / (float)HW, os,
+                                                                               count);
       TFB_CHECK_LAUNCH();
       return TFB_OK;
     }
@@ -856,14 +926,14 @@ TFB_API int tfb_bn_fwd_stats(const float* x, float* y, int64_t M, int C, const f
     const int rc = ordered_alloc(os, splits, (int64_t)pool_batch * C, stream);
     if (rc != TFB_OK) return rc;
     bn_apply_pool_stats_kernel<<<grid, block, 0, stream>>>(x, y, HW, C, M, stats, gamma, beta, eps, momentum, relu, save_mean, save_invstd,
-                                                              running_mean, running_var, pooled, 1.f / (float)HW, os);
+                                                              running_mean, running_var, pooled, 1.f / (float)HW, os, count);
     TFB_CHECK_LAUNCH();
     return TFB_OK;
   }
   const int64_t total4 = M * C / 4;
   bn_apply_stats_kernel<<<tfb_grid(total4, 256, 4), 256, 0, stream>>>(x, y, total4, C, M, stats, gamma, beta, eps, momentum, relu, save_mean,
                                                                          save_invstd, running_mean, running_var,
-                                                                         (__nv_bfloat16*)y16_bf16, residual);
+                                                                         (__nv_bfloat16*)y16_bf16, residual, count);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
@@ -879,22 +949,12 @@ TFB_API int tfb_bn_apply(const float* x, float* y, int64_t M, int C, const float
   return TFB_OK;
 }
 
-// Common body of tfb_bn_bwd / tfb_bn_bwd_se: column reduction (sum g, sum g*xhat per channel) + apply pass.
-static int bn_bwd_impl(const float* x, const float* dy, float* dx, int64_t M, int C, const float* gamma, const float* beta,
-                       const float* save_mean, const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws,
-                       void* dx16_bf16, const float* ymask, float* gmasked, const float* se_gate, const float* se_dpool, int hw,
-                       cudaStream_t stream) {
+// The column reduction of BatchNorm backward (sum g, sum g*xhat per channel) -> dbeta, dgamma; slice (optional): the same sums in fp64.
+static int bn_bwd_reduce(const float* x, const float* dy, int64_t M, int C, const float* gamma, const float* beta, const float* save_mean,
+                         const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws, const float* ymask,
+                         const float* se_gate, const float* se_dpool, int hw, double* slice, cudaStream_t stream) {
   Finalize fin = {2, 2 * C, M, 0.f, 0.f, dbeta, dgamma, nullptr, nullptr};
-  const bool vec = aligned16(x) && aligned16(dy) && aligned16(dx) && (!ymask || aligned16(ymask)) && (!se_gate || (aligned16(se_gate) && aligned16(se_dpool)));
-  if (se_gate && !vec) {
-    // unaligned operands (never the case for the trunks' maps): the squeeze-excite gradient as its own pass (into dx, which the
-    // BatchNorm passes then read as dy and overwrite element by element)
-    const int64_t total = M * C;
-    scale_gate_kernel<<<tfb_grid(total / 4, 256), 256, 0, stream>>>(dy, se_gate, se_dpool, 1.f / (float)hw, dx, total / 4, hw, C);
-    TFB_CHECK_LAUNCH();
-    dy = dx;
-    se_gate = se_dpool = nullptr;
-  }
+  fin.slice = slice;
   if (se_gate) {
     int rc;
     if (C / 4 <= 128 && M >= 4096) {            // as launch_colreduce picks
@@ -918,8 +978,30 @@ static int bn_bwd_impl(const float* x, const float* dy, float* dx, int64_t M, in
     const int rc = launch_colreduce<1>(x, C, dy, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu, ymask, fin, stream);
     if (rc != TFB_OK) return rc;
   }
+  return TFB_OK;
+}
+
+// Common body of tfb_bn_bwd / tfb_bn_bwd_se: column reduction (sum g, sum g*xhat per channel) + apply pass.
+static int bn_bwd_impl(const float* x, const float* dy, float* dx, int64_t M, int C, const float* gamma, const float* beta,
+                       const float* save_mean, const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws,
+                       void* dx16_bf16, const float* ymask, float* gmasked, const float* se_gate, const float* se_dpool, int hw,
+                       cudaStream_t stream) {
+  const bool vec = aligned16(x) && aligned16(dy) && aligned16(dx) && (!ymask || aligned16(ymask)) && (!se_gate || (aligned16(se_gate) && aligned16(se_dpool)));
+  if (se_gate && !vec) {
+    // unaligned operands (never the case for the trunks' maps): the squeeze-excite gradient as its own pass (into dx, which the
+    // BatchNorm passes then read as dy and overwrite element by element)
+    const int64_t total = M * C;
+    scale_gate_kernel<<<tfb_grid(total / 4, 256), 256, 0, stream>>>(dy, se_gate, se_dpool, 1.f / (float)hw, dx, total / 4, hw, C);
+    TFB_CHECK_LAUNCH();
+    dy = dx;
+    se_gate = se_dpool = nullptr;
+  }
+  const int rc = bn_bwd_reduce(x, dy, M, C, gamma, beta, save_mean, save_invstd, relu, dgamma, dbeta, sums_ws, ymask, se_gate, se_dpool, hw,
+                               nullptr, stream);
+  if (rc != TFB_OK) return rc;
   bn_bwd_apply_kernel<<<tfb_grid(M * C / 4, 256), 256, 0, stream>>>(x, dy, dx, M, C, sums_ws, save_mean, save_invstd, gamma, beta, relu,
-                                                                dgamma, dbeta, (__nv_bfloat16*)dx16_bf16, ymask, gmasked, se_gate, se_dpool, hw);
+                                                                dgamma, dbeta, (__nv_bfloat16*)dx16_bf16, ymask, gmasked, se_gate, se_dpool, hw,
+                                                                nullptr);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
@@ -951,6 +1033,75 @@ TFB_API int tfb_bn_bwd_se(const float* x, const float* dy, float* dx, int64_t M,
   TFB_REQUIRE(se_gate && se_dpool && hw > 0 && M % hw == 0 && M < (int64_t)1 << 31);
   return bn_bwd_impl(x, dy, dx, M, C, gamma, beta, save_mean, save_invstd, relu, dgamma, dbeta, sums_ws, dx16_bf16, nullptr, nullptr,
                      se_gate, se_dpool, hw, stream);
+}
+
+// Synchronized BatchNorm (torch.nn.SyncBatchNorm semantics over the ranks of a process group), forward, step 1 of 2: this rank's
+// slice = [sum x | sum x^2 | M] (2*C + 1 doubles). stats (optional): the sums the producing conv / GEMM epilogue accumulated (as for
+// tfb_bn_fwd_stats), copied; else one statistics pass over x (sums_ws as for tfb_bn_fwd). The caller gathers the W ranks' slices.
+TFB_API int tfb_bn_sync_slice(const float* x, int64_t M, int C, const double* stats, double* slice, double* sums_ws, cudaStream_t stream) {
+  TFB_REQUIRE(slice && M > 0 && C > 0 && C % 4 == 0 && (stats || (x && sums_ws)));
+  if (stats) {
+    bn_sync_slice_copy_kernel<<<(2 * C + 256) / 256, 256, 0, stream>>>(stats, C, M, slice);
+    TFB_CHECK_LAUNCH();
+    return TFB_OK;
+  }
+  Finalize fin = {4, 2 * C, M, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr};
+  fin.slice = slice;
+  return launch_colreduce<0>(x, C, nullptr, M, C, sums_ws, nullptr, nullptr, nullptr, nullptr, 0, nullptr, fin, stream);
+}
+
+// Synchronized BatchNorm forward, step 2 of 2: gathered = the W ranks' slices [W][2*C + 1] in rank order. Folds them in rank order
+// (folded: the sums and the total count N, 2*C + 1 doubles, kept for backward), then normalises with the global mean / biased variance;
+// the running statistics take the unbiased variance over N. from_stats = 0: the normalise pass of tfb_bn_fwd, 1: that of
+// tfb_bn_fwd_stats (with one rank, the same bits as that entry point). pooled (optional): cleared here, then accumulated.
+// Everything else as tfb_bn_fwd.
+TFB_API int tfb_bn_fwd_sync(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, float eps, float momentum,
+                            int relu, float* running_mean, float* running_var, float* save_mean, float* save_invstd, const double* gathered,
+                            int world, double* folded, int from_stats, void* y16_bf16, const float* residual, float* pooled, int pool_batch,
+                            cudaStream_t stream) {
+  TFB_REQUIRE(x && y && gamma && beta && save_mean && save_invstd && gathered && folded && world > 0 && M > 0 && C > 0 && C % 4 == 0);
+  TFB_REQUIRE(!pooled || (pool_batch > 0 && M % pool_batch == 0 && !y16_bf16 && !residual));
+  TFB_REQUIRE(!from_stats || C <= kBnStatsMaxC);
+  bn_sync_fold_kernel<<<(C + 255) / 256, 256, 0, stream>>>(gathered, world, C, 1, eps, momentum, save_mean, save_invstd, running_mean,
+                                                           running_var, folded, nullptr, pooled, pooled ? pool_batch * C : 0);
+  TFB_CHECK_LAUNCH();
+  if (from_stats)
+    return bn_apply_stats_launch(x, y, M, C, gamma, beta, eps, momentum, relu, nullptr, nullptr, save_mean, save_invstd, folded, folded + 2 * C,
+                                 y16_bf16, residual, pooled, pool_batch, stream);
+  return bn_apply_launch(x, y, M, C, gamma, beta, relu, save_mean, save_invstd, y16_bf16, residual, pooled, pool_batch, stream);
+}
+
+// Synchronized BatchNorm backward, step 1 of 2: the reduction pass of tfb_bn_bwd (ymask) / tfb_bn_bwd_se (se_gate, se_dpool, hw),
+// writing this rank's dgamma / dbeta (local, as torch.nn.SyncBatchNorm returns them) and its slice = [sum g | sum g*xhat] (2*C doubles).
+// Operands 16-byte aligned when se_gate is given.
+TFB_API int tfb_bn_bwd_sync_reduce(const float* x, const float* dy, int64_t M, int C, const float* gamma, const float* beta, const float* save_mean,
+                                   const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws, const float* ymask,
+                                   const float* se_gate, const float* se_dpool, int hw, double* slice, cudaStream_t stream) {
+  TFB_REQUIRE(x && dy && gamma && beta && save_mean && save_invstd && dgamma && dbeta && sums_ws && slice && M > 0 && C > 0 && C % 4 == 0);
+  TFB_REQUIRE(!se_gate || (se_dpool && hw > 0 && M % hw == 0 && M < (int64_t)1 << 31 && !ymask && aligned16(x) && aligned16(dy) &&
+                           aligned16(se_gate) && aligned16(se_dpool)));
+  return bn_bwd_reduce(x, dy, M, C, gamma, beta, save_mean, save_invstd, relu, dgamma, dbeta, sums_ws, ymask, se_gate, se_dpool, hw, slice,
+                       stream);
+}
+
+// Synchronized BatchNorm backward, step 2 of 2: gathered = the W ranks' slices [W][2*C] in rank order, folded in rank order into
+// gsum (2*C floats of scratch: [sum g | sum g*xhat] over every rank); count = the total row count N of the forward (folded[2*C] of
+// tfb_bn_fwd_sync). dx = gamma * invstd * (g - sum_g/N - xhat * sum_gx/N); dx16_bf16 / ymask / gmasked / se_* as for tfb_bn_bwd(_se).
+TFB_API int tfb_bn_bwd_sync_apply(const float* x, const float* dy, float* dx, int64_t M, int C, const float* gamma, const float* beta,
+                                  const float* save_mean, const float* save_invstd, int relu, const double* gathered, int world, const double* count,
+                                  float* gsum, void* dx16_bf16, const float* ymask, float* gmasked, const float* se_gate, const float* se_dpool,
+                                  int hw, cudaStream_t stream) {
+  TFB_REQUIRE(x && dy && dx && gamma && beta && save_mean && save_invstd && gathered && count && gsum && world > 0 && M > 0 && C > 0 &&
+              C % 4 == 0);
+  TFB_REQUIRE((!gmasked || ymask) && (!se_gate || (se_dpool && hw > 0 && M % hw == 0 && M < (int64_t)1 << 31)));
+  bn_sync_fold_kernel<<<(C + 255) / 256, 256, 0, stream>>>(gathered, world, C, 0, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, gsum,
+                                                           nullptr, 0);
+  TFB_CHECK_LAUNCH();
+  bn_bwd_apply_kernel<<<tfb_grid(M * C / 4, 256), 256, 0, stream>>>(x, dy, dx, M, C, nullptr, save_mean, save_invstd, gamma, beta, relu,
+                                                                gsum + C, gsum, (__nv_bfloat16*)dx16_bf16, ymask, gmasked, se_gate, se_dpool, hw,
+                                                                count);
+  TFB_CHECK_LAUNCH();
+  return TFB_OK;
 }
 
 // out[c] = sum_r x[r][c]  (bias gradients of Linear / 1x1 conv layers)

@@ -8,6 +8,7 @@ import os
 import weakref
 
 import torch
+import torch.distributed as dist
 from torch.autograd import Function
 
 from . import _lib
@@ -72,10 +73,95 @@ def tick(device):
     if a['off'] > 0:
         a['buf'][:a['off']].zero_()          # what the last step handed out; everything beyond is still zero
     a['off'] = 0
+    s = _SYNC.get(dev)
+    if s is not None:
+        s['chunk'], s['off'] = 0, 0
     _SEED['off'] = 0
     _BWD16.clear()
     _COL_CACHE.clear()
     _prepack_all(device)
+
+
+# Per-step arena of the synchronized BatchNorms' fp64 slices (a rank's [sum x | sum x^2 | count] / [sum g | sum g*xhat], the W gathered
+# slices, the folded sums): handed out in call order and rewound by tick(), so every step and a captured CUDA graph use the same
+# addresses. Grown by whole chunks (kept for good) when a step needs more; nothing here is read before it is written.
+_SYNC = {}
+SYNC_CHUNK_BYTES = 4 << 20
+
+
+def _sync_take(device, n, dtype=torch.float64):
+    dev = torch.device(device)
+    a = _SYNC.setdefault(dev, dict(chunks=[], chunk=0, off=0))
+    item = torch.empty(0, dtype=dtype).element_size()
+    nbytes = (n * item + 15) // 16 * 16
+    while True:
+        if a['chunk'] == len(a['chunks']):
+            a['chunks'].append(torch.empty(max(SYNC_CHUNK_BYTES, nbytes), dtype=torch.uint8, device=dev))
+        buf = a['chunks'][a['chunk']]
+        if a['off'] + nbytes <= buf.numel():
+            break
+        a['chunk'], a['off'] = a['chunk'] + 1, 0
+    off, a['off'] = a['off'], a['off'] + nbytes
+    return torch.empty(0, dtype=dtype, device=dev).set_(buf.untyped_storage(), off // item, (n,))
+
+
+def sync_group(bn):
+    """The process group a training-mode BatchNorm normalises over: that of an nn.SyncBatchNorm (its `process_group`, WORLD when
+    None) once a default process group exists, else None (per-rank statistics, plain nn.BatchNorm2d)."""
+    if not isinstance(bn, torch.nn.SyncBatchNorm) or not (dist.is_available() and dist.is_initialized()):
+        return None
+    return bn.process_group if bn.process_group is not None else dist.group.WORLD
+
+
+def _gather_slices(slice_, group):
+    """[W * n] = the n-value slices of the W ranks of `group`, in rank order (all-gather: every rank then folds the same values in the
+    same order, whatever algorithm the collective uses). gloo gathers CUDA tensors through host memory."""
+    W = dist.get_world_size(group)
+    out = _sync_take(slice_.device, W * slice_.numel())
+    if slice_.is_cuda and dist.get_backend(group) == 'gloo':
+        host = torch.empty(W * slice_.numel(), dtype=slice_.dtype)
+        dist.all_gather_into_tensor(host, slice_.cpu(), group=group)
+        out.copy_(host)
+    else:
+        dist.all_gather_into_tensor(out, slice_, group=group)
+    return out, W
+
+
+def _bn_fwd(x, y, M, C, weight, bias, momentum, eps, relu, running_mean, running_var, mean, invstd, stats, y16, residual, pooled,
+            pool_batch, group):
+    """Training-mode BatchNorm forward (see batch_norm); returns the synchronized BatchNorm's folded sums + total count, or None."""
+    if group is None:
+        if stats is not None:
+            call('tfb_bn_fwd_stats', x, y, M, C, weight, bias, float(eps), float(momentum), int(relu), running_mean, running_var, mean, invstd,
+                 stats, y16, residual, pooled, pool_batch)
+        else:
+            call('tfb_bn_fwd', x, y, M, C, weight, bias, float(eps), float(momentum), int(relu), running_mean, running_var, mean, invstd,
+                 _ws(x.device), y16, residual, pooled, pool_batch)
+        return None
+    sl = _sync_take(x.device, 2 * C + 1)
+    call('tfb_bn_sync_slice', x, M, C, stats, sl, _ws(x.device))
+    g, W = _gather_slices(sl, group)
+    folded = _sync_take(x.device, 2 * C + 1)
+    call('tfb_bn_fwd_sync', x, y, M, C, weight, bias, float(eps), float(momentum), int(relu), running_mean, running_var, mean, invstd, g, W,
+         folded, int(stats is not None), y16, residual, pooled, pool_batch)
+    return folded
+
+
+def _bn_bwd(x, dy, dx, M, C, weight, bias, mean, invstd, relu, dg, db, dx16, ymask=None, gmasked=None, se_gate=None, se_dpool=None, hw=1,
+            group=None, folded=None):
+    """Training-mode BatchNorm backward; `folded` / `group` from the synchronized forward (_bn_fwd)."""
+    if group is None:
+        if se_gate is not None:
+            call('tfb_bn_bwd_se', x, dy, dx, M, C, weight, bias, mean, invstd, int(relu), dg, db, _ws(x.device), dx16, se_gate, se_dpool, hw)
+        else:
+            call('tfb_bn_bwd', x, dy, dx, M, C, weight, bias, mean, invstd, int(relu), dg, db, _ws(x.device), dx16, ymask, gmasked)
+        return
+    sl = _sync_take(x.device, 2 * C)
+    call('tfb_bn_bwd_sync_reduce', x, dy, M, C, weight, bias, mean, invstd, int(relu), dg, db, _ws(x.device), ymask, se_gate, se_dpool, hw, sl)
+    g, W = _gather_slices(sl, group)
+    gsum = _sync_take(x.device, 2 * C, torch.float32)
+    call('tfb_bn_bwd_sync_apply', x, dy, dx, M, C, weight, bias, mean, invstd, int(relu), g, W, folded[2 * C:], gsum, dx16, ymask, gmasked,
+         se_gate, se_dpool, hw)
 
 
 def next_seed():
@@ -955,7 +1041,8 @@ class BatchNormTrainFn(Function):
     """BatchNorm2d in training mode (+ fused ReLU): batch statistics, running-stat update (momentum, unbiased var)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, relu, emit16=False, bwd16=False, pool=False, stats=None):
+    def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, relu, emit16=False, bwd16=False, pool=False, stats=None,
+                group=None):
         x = _c(x)
         C = x.shape[-1]
         M = x.numel() // C
@@ -972,36 +1059,31 @@ class BatchNormTrainFn(Function):
                 stats = None
             else:
                 pooled = pooled.view(x.shape[0], C)
-        if stats is not None:
-            # the conv / GEMM that produced x already accumulated sum x, sum x^2 per channel in its epilogue: one launch, one pass
-            call('tfb_bn_fwd_stats', x, y, M, C, weight, bias, float(eps), float(momentum), int(relu), running_mean, running_var, mean, invstd,
-                 stats, y16, None, pooled, x.shape[0] if pool else 0)
-        else:
-            if pool:
-                pooled = torch.empty((x.shape[0], C), dtype=torch.float32, device=x.device)
-            call('tfb_bn_fwd', x, y, M, C, weight, bias, float(eps), float(momentum), int(relu), running_mean, running_var, mean, invstd,
-                 _ws(x.device), y16, None, pooled, x.shape[0] if pool else 0)
-        ctx.save_for_backward(x, weight, bias, mean, invstd)
-        ctx.relu, ctx.bwd16 = relu, bwd16
+        if stats is None and pool:
+            pooled = torch.empty((x.shape[0], C), dtype=torch.float32, device=x.device)
+        # stats: the conv / GEMM that produced x already accumulated sum x, sum x^2 per channel in its epilogue: one launch, one pass
+        folded = _bn_fwd(x, y, M, C, weight, bias, momentum, eps, relu, running_mean, running_var, mean, invstd, stats, y16, None, pooled,
+                         x.shape[0] if pool else 0, group)
+        ctx.save_for_backward(x, weight, bias, mean, invstd, folded)
+        ctx.relu, ctx.bwd16, ctx.group = relu, bwd16, group
         if pool:
             y._tfb_pooled = pooled
         return _attach16(y, y16)
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, bias, mean, invstd = ctx.saved_tensors
+        x, weight, bias, mean, invstd, folded = ctx.saved_tensors
         dy = _c(dy)
         C = x.shape[-1]
         M = x.numel() // C
         dx = torch.empty_like(x)
         dg = _gbuf(weight)
         db = _gbuf(bias)
-        ws = _ws(x.device)
         dx16 = _emit16(dx, ctx.bwd16)
-        call('tfb_bn_bwd', x, dy, dx, M, C, weight, bias, mean, invstd, int(ctx.relu), dg, db, ws, dx16, None, None)
+        _bn_bwd(x, dy, dx, M, C, weight, bias, mean, invstd, ctx.relu, dg, db, dx16, group=ctx.group, folded=folded)
         if dx16 is not None:
             _offer16(dx, dx16)
-        return dx, dg, db, None, None, None, None, None, None, None, None, None
+        return dx, dg, db, None, None, None, None, None, None, None, None, None, None
 
 
 class BatchNormAddReluFn(Function):
@@ -1010,7 +1092,7 @@ class BatchNormAddReluFn(Function):
     passes — two launches and four passes over the block-sized activation fewer than BatchNorm, add+ReLU, ReLU', BatchNorm'."""
 
     @staticmethod
-    def forward(ctx, x, res, weight, bias, running_mean, running_var, momentum, eps, emit16=False, bwd16=False, stats=None):
+    def forward(ctx, x, res, weight, bias, running_mean, running_var, momentum, eps, emit16=False, bwd16=False, stats=None, group=None):
         x, res = _c(x), _c(res)
         C = x.shape[-1]
         M = x.numel() // C
@@ -1018,33 +1100,29 @@ class BatchNormAddReluFn(Function):
         y16 = _emit16(y, emit16)
         mean = torch.empty(C, dtype=torch.float32, device=x.device)
         invstd = torch.empty(C, dtype=torch.float32, device=x.device)
-        if stats is not None:
-            call('tfb_bn_fwd_stats', x, y, M, C, weight, bias, float(eps), float(momentum), 1, running_mean, running_var, mean, invstd,
-                 stats, y16, res, None, 0)
-        else:
-            call('tfb_bn_fwd', x, y, M, C, weight, bias, float(eps), float(momentum), 1, running_mean, running_var, mean, invstd,
-                 _ws(x.device), y16, res, None, 0)
-        ctx.save_for_backward(x, weight, bias, mean, invstd, y)
-        ctx.bwd16 = bwd16
+        folded = _bn_fwd(x, y, M, C, weight, bias, momentum, eps, 1, running_mean, running_var, mean, invstd, stats, y16, res, None, 0, group)
+        ctx.save_for_backward(x, weight, bias, mean, invstd, y, folded)
+        ctx.bwd16, ctx.group = bwd16, group
         return _attach16(y, y16)
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, bias, mean, invstd, y = ctx.saved_tensors
+        x, weight, bias, mean, invstd, y, folded = ctx.saved_tensors
         dy = _c(dy)
         C = x.shape[-1]
         M = x.numel() // C
         dx, g = torch.empty_like(x), torch.empty_like(x)
         dg, db = _gbuf(weight), _gbuf(bias)
         dx16 = _emit16(dx, ctx.bwd16)
-        call('tfb_bn_bwd', x, dy, dx, M, C, weight, bias, mean, invstd, 0, dg, db, _ws(x.device), dx16, y, g)
+        _bn_bwd(x, dy, dx, M, C, weight, bias, mean, invstd, 0, dg, db, dx16, ymask=y, gmasked=g, group=ctx.group, folded=folded)
         if dx16 is not None:
             _offer16(dx, dx16)
-        return dx, g, dg, db, None, None, None, None, None, None, None
+        return dx, g, dg, db, None, None, None, None, None, None, None, None
 
 
 def batch_norm(x, bn, relu, training, emit16=False, bwd16=False, residual=None, pool=False):
-    """bn: an nn.BatchNorm2d used as a parameter/buffer container. residual: act(bn(x) + residual) in the same pass (relu required).
+    """bn: an nn.BatchNorm2d used as a parameter/buffer container; an nn.SyncBatchNorm in training mode normalises with the
+    statistics of all ranks of its process group once one is initialised (sync_group). residual: act(bn(x) + residual) in the same pass (relu required).
     pool: the output feeds a squeeze-excite module next — its global average pool is accumulated in the normalise pass (training). emit16: the output feeds a tensor-core GEMM / conv next, so
     (bf16 mode) its bf16 copy is written in the same pass. bwd16: the same for dx in backward (the convolution in front of this
     BatchNorm has no bias / ReLU of its own and runs dgrad + wgrad on the tensor cores)."""
@@ -1054,11 +1132,12 @@ def batch_norm(x, bn, relu, training, emit16=False, bwd16=False, residual=None, 
         stats = getattr(x, '_tfb_stats', None)        # accumulated by the producing conv / GEMM epilogue (conv2d(..., bn_stats=True))
         if stats is not None and (stats.numel() != 2 * x.shape[-1] or x.shape[-1] > 2048):
             stats = None
+        group = sync_group(bn)
         if residual is not None:
             return BatchNormAddReluFn.apply(x, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.momentum, bn.eps, emit16,
-                                            bwd16, stats)
+                                            bwd16, stats, group)
         return BatchNormTrainFn.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.momentum, bn.eps, relu, emit16, bwd16,
-                                      pool, stats)
+                                      pool, stats, group)
     if torch.is_grad_enabled() and x.requires_grad:
         raise RuntimeError('eval-mode BatchNorm backward is not implemented (training path only)')
     C = x.shape[-1]
@@ -1175,7 +1254,7 @@ class BNSEFn(Function):
     launch, one write and one read of the block-sized map fewer per bottleneck."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, w1, b1, w2, b2, bwd16, stats):
+    def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, w1, b1, w2, b2, bwd16, stats, group=None):
         x = _c(x)
         N, H, W, C = x.shape
         M, Cr, dev = N * H * W, w1.shape[0], x.device
@@ -1186,13 +1265,9 @@ class BNSEFn(Function):
         if stats is not None:
             pooled = _arena_take(dev, N * C * 4, torch.float32)               # accumulated into: must start at zero
             pooled = pooled.view(N, C) if pooled is not None else None
-        if stats is not None and pooled is not None:
-            call('tfb_bn_fwd_stats', x, y2, M, C, weight, bias, float(eps), float(momentum), 1, running_mean, running_var, mean, invstd,
-                 stats, None, None, pooled, N)
-        else:
-            pooled = torch.empty((N, C), dtype=torch.float32, device=dev)
-            call('tfb_bn_fwd', x, y2, M, C, weight, bias, float(eps), float(momentum), 1, running_mean, running_var, mean, invstd,
-                 _ws(dev), None, None, pooled, N)
+        if pooled is None:
+            stats, pooled = None, torch.empty((N, C), dtype=torch.float32, device=dev)
+        folded = _bn_fwd(x, y2, M, C, weight, bias, momentum, eps, 1, running_mean, running_var, mean, invstd, stats, None, None, pooled, N, group)
         h = torch.empty((N, Cr), dtype=torch.float32, device=dev)
         gate = torch.empty((N, C), dtype=torch.float32, device=dev)
         call('tfb_gemm_small_m', 1, N, Cr, C, pooled, C, w1, C, h, Cr, b1, 1)
@@ -1200,13 +1275,13 @@ class BNSEFn(Function):
         y = torch.empty_like(x)
         y16 = _emit16(y, True)                               # the gated output always feeds the 1x1 conv3 GEMM
         call('tfb_se_scale_fwd', y2, gate, y, N, H * W, C, y16)
-        ctx.save_for_backward(x, weight, bias, mean, invstd, y2, w1, w2, pooled, h, gate, b1, b2)
-        ctx.bwd16 = bwd16
+        ctx.save_for_backward(x, weight, bias, mean, invstd, y2, w1, w2, pooled, h, gate, b1, b2, folded)
+        ctx.bwd16, ctx.group = bwd16, group
         return _attach16(y, y16)
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, bias, mean, invstd, y2, w1, w2, pooled, h, gate, b1, b2 = ctx.saved_tensors
+        x, weight, bias, mean, invstd, y2, w1, w2, pooled, h, gate, b1, b2, folded = ctx.saved_tensors
         dy = _c(dy)
         N, H, W, C = x.shape
         M, Cr, dev = N * H * W, w1.shape[0], x.device
@@ -1219,10 +1294,11 @@ class BNSEFn(Function):
         dx = torch.empty_like(x)
         dg, db = _gbuf(weight), _gbuf(bias)
         dx16 = _emit16(dx, ctx.bwd16)
-        call('tfb_bn_bwd_se', x, dy, dx, M, C, weight, bias, mean, invstd, 1, dg, db, _ws(dev), dx16, gate, dpool, H * W)
+        _bn_bwd(x, dy, dx, M, C, weight, bias, mean, invstd, 1, dg, db, dx16, se_gate=gate, se_dpool=dpool, hw=H * W, group=ctx.group,
+                folded=folded)
         if dx16 is not None:
             _offer16(dx, dx16)
-        return dx, dg, db, None, None, None, None, dw1, db1, dw2, db2, None, None
+        return dx, dg, db, None, None, None, None, dw1, db1, dw2, db2, None, None, None
 
 
 def bn_se_ok(x, bn, fc1):
@@ -1237,7 +1313,7 @@ def bn_se(x, bn, fc1, fc2, bwd16=False):
     if stats is not None and (stats.numel() != 2 * x.shape[-1] or x.shape[-1] > 2048):
         stats = None
     return BNSEFn.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.momentum, bn.eps, fc1.weight, fc1.bias, fc2.weight,
-                        fc2.bias, bwd16, stats)
+                        fc2.bias, bwd16, stats, sync_group(bn))
 
 
 class AddFn(Function):

@@ -26,7 +26,12 @@ DATASET_KEYS = tuple(k for k in RAW_KEYS if k != 'bev') + ('n_valid', 'bev_u8', 
 
 class Trainer:
     def __init__(self, cfg, device, gemm_mode='bf16', lr=1e-4, seed=0, n_chunks=int(os.environ.get('TFB_GRAD_CHUNKS', '8')), backbone='transFuser',
-                 raw_inputs=False, image_architecture='regnety_032', lidar_architecture='regnety_032', use_velocity=False):
+                 raw_inputs=False, image_architecture='regnety_032', lidar_architecture='regnety_032', use_velocity=False,
+                 sync_batch_norm=False):
+        """sync_batch_norm: every BatchNorm normalises with the statistics of the global batch (train.py --sync_batch_norm 1): the model
+        is converted with nn.SyncBatchNorm.convert_sync_batchnorm and each trunk's BatchNorms get a process group of their own, apart
+        from the gradient all-reduce's, so one trunk's statistics never queue behind the other trunk's or behind the gradients. Needs an
+        initialised default process group (world size 1 included)."""
         self.cfg, self.device = cfg, device
         self.raw_inputs = raw_inputs
         if raw_inputs not in (False, True, 'dataset'):
@@ -43,6 +48,15 @@ class Trainer:
         gemm.set_mode(gemm_mode)
         ops.manual_seed(1234 + seed)
         self.net = LidarCenterNet(cfg, device, backbone, image_architecture, lidar_architecture, use_velocity=use_velocity).train()
+        if sync_batch_norm:
+            if not dist.is_initialized():
+                raise RuntimeError('sync_batch_norm=True needs an initialised process group (torch.distributed.init_process_group)')
+            self.net = torch.nn.SyncBatchNorm.convert_sync_batchnorm(self.net)
+            # new_group is collective: every rank creates both groups here, before any step is captured
+            groups = {'image': dist.new_group(), 'lidar': dist.new_group()}
+            for name, m in self.net.named_modules():
+                if isinstance(m, torch.nn.SyncBatchNorm):
+                    m.process_group = groups['lidar' if 'lidar_encoder' in name else 'image']
         self.flat = optim.flatten(self.net)
         if self.world > 1:
             # replicas start identical whatever the caller's RNG state: rank 0's parameters and buffers win (DDP does the same at
