@@ -17,6 +17,7 @@ import torch
 U32 = 0xFFFFFFFF
 EPS32 = 2.0 ** -23          # 2u of fp32 (u = 2^-24): the per-add bound used throughout
 TINY = 1e-30
+SENT = -1024.0              # sentinel behind every Guarded output (exactly representable in bf16 and fp32)
 
 
 def bf(x):
@@ -70,6 +71,27 @@ def check(out, ref, mag, K, tol, slack=None, what='', floor=0.0):
                                 int((err > allow).sum()), rel))
     assert rel <= tol, '%s: relative L2 %.3g > %.3g' % (what, rel, tol)
     return rel, ratio
+
+
+class Guarded:
+    """A NaN-filled output tensor followed by sentinel elements that must stay bit-unchanged."""
+
+    def __init__(self, shape, dtype, device='cuda'):
+        n = math.prod(shape)
+        self.buf = torch.empty(n + 64, dtype=dtype, device=device)
+        self.t = self.buf[:n].view(shape)
+        self.n = n
+
+    def reset(self):
+        self.buf[self.n:].fill_(SENT)
+        self.t.fill_(float('nan'))
+        return self.t
+
+    def tail_ok(self):
+        return bool((self.buf[self.n:] == SENT).all())
+
+    def bits(self):
+        return self.buf.clone().view(torch.int16 if self.buf.dtype == torch.bfloat16 else torch.int32)
 
 
 # ------------------------------------------------------------------ attention dropout mask (csrc/attn_tc.cu drop_scale)

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_tc_exact import Guarded
+from tc_ref import Guarded
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'

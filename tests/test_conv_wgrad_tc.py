@@ -14,7 +14,8 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import tc_ref as R  # noqa: E402
-from test_tc_exact import Guarded, _call  # noqa: E402
+from tc_ref import Guarded  # noqa: E402
+from test_tc_exact import _call  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'

@@ -53,6 +53,8 @@ def test_sync_kernels_simulated_ranks(world, variant, from_stats):
     from transfuser_b200 import _lib
     sync_bn_check.run(_lib.call, 'cuda', world, variant, from_stats, C=72, hw=40)
     sync_bn_check.run(_lib.call, 'cuda', world, variant, from_stats, C=1512, hw=3)
+    if world == 1:      # rank 0 holds 3 samples: M = 4200 rows, the flat statistics / reduction kernels
+        sync_bn_check.run(_lib.call, 'cuda', world, variant, from_stats, C=72, hw=1400)
 
 
 def _snapshot(tr, loss):

@@ -15,6 +15,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import tc_ref as R  # noqa: E402
+from tc_ref import Guarded  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -25,34 +26,12 @@ ATTN_TOL = 1e-3
 ATTN16_TOL = 4e-3
 CONV_TOL = 7e-5          # 10x the measured worst, 7.1e-6 (dw of the 1056-tile case)
 PLAIN_TOL = 2e-2         # against the plain fp64 references (no rounding): a bound on bf16-operand error, not on the kernel
-SENT = -1024.0
 SEED = 0x5EED1234ABCD
 
 
 def _call(name, *a):
     from transfuser_b200 import _lib
     _lib.call(name, *a)
-
-
-class Guarded:
-    """A NaN-filled output tensor followed by sentinel elements that must stay bit-unchanged."""
-
-    def __init__(self, shape, dtype):
-        n = math.prod(shape)
-        self.buf = torch.empty(n + 64, dtype=dtype, device=DEV)
-        self.t = self.buf[:n].view(shape)
-        self.n = n
-
-    def reset(self):
-        self.buf[self.n:].fill_(SENT)
-        self.t.fill_(float('nan'))
-        return self.t
-
-    def tail_ok(self):
-        return bool((self.buf[self.n:] == SENT).all())
-
-    def bits(self):
-        return self.buf.clone().view(torch.int16 if self.buf.dtype == torch.bfloat16 else torch.int32)
 
 
 # ------------------------------------------------------------------ attention

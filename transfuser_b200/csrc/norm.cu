@@ -769,20 +769,11 @@ __global__ void __launch_bounds__(256) bn_sync_slice_copy_kernel(const double* _
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= 2 * C; i += gridDim.x * blockDim.x) slice[i] = i < 2 * C ? stats[i] : (double)M;
 }
 
-// d[n, hw, c] = dy * gate[n][c] + dpool[n][c] * inv_hw  (float4 per thread; C % 4 == 0)
-__global__ void __launch_bounds__(256) scale_gate_kernel(const float* __restrict__ dy, const float* __restrict__ gate,
-                                                         const float* __restrict__ dpool, float inv_hw, float* __restrict__ d, int64_t total4,
-                                                         int hw, int C) {
-  const int C4 = C / 4;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (int64_t)gridDim.x * blockDim.x) {
-    const float4 v = reinterpret_cast<const float4*>(dy)[i];
-    float g[4] = {v.x, v.y, v.z, v.w};
-    se_grad4(g, gate, dpool, (int64_t)((int)(i / C4) / hw) * C + (int)(i % C4) * 4, inv_hw);
-    reinterpret_cast<float4*>(d)[i] = make_float4(g[0], g[1], g[2], g[3]);
-  }
-}
-
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+// Alignment of the operands the BatchNorm apply passes access as float4 (16 bytes) and of the bf16 sidecars they store four at a time
+// (8 bytes); a null optional operand passes.
+inline bool opt16(const void* p) { return !p || aligned16(p); }
+inline bool opt8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
 
 // fin.part for a reduction with nsplit row splits and fin.cnt for `slabs` channel slabs, in the stream's scratch.
 int alloc_partials(Finalize& fin, int64_t nsplit, int slabs, cudaStream_t stream) {
@@ -853,11 +844,15 @@ static int bn_apply_stats_launch(const float* x, float* y, int64_t M, int C, con
 // pooled (optional, [pool_batch, C], M = pool_batch * HW): also the squeeze-excite pooling of the output, pooled[n][c] =
 // mean over the HW pixels of sample n of y — cleared by the statistics kernel, accumulated by the apply kernel (no memset, no
 // separate pooling pass); excludes y16_bf16 / residual.
+// x, y, residual, gamma, beta, save_mean and save_invstd 16-byte aligned, y16_bf16 8-byte aligned (the normalise pass reads and
+// writes four channels at a time); other operands are refused.
 TFB_API int tfb_bn_fwd(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, float eps,
                        float momentum, int relu, float* running_mean, float* running_var, float* save_mean, float* save_invstd,
                        double* sums_ws, void* y16_bf16, const float* residual, float* pooled, int pool_batch, cudaStream_t stream) {
   TFB_REQUIRE(x && y && gamma && beta && save_mean && save_invstd && sums_ws && M > 0 && C > 0 && C % 4 == 0);
   TFB_REQUIRE(!pooled || (pool_batch > 0 && M % pool_batch == 0 && !y16_bf16 && !residual));
+  TFB_REQUIRE(aligned16(x) && aligned16(y) && opt16(residual) && opt8(y16_bf16) && aligned16(gamma) && aligned16(beta) && aligned16(save_mean) &&
+              aligned16(save_invstd));
   Finalize fin = {1, 2 * C, M, eps, momentum, save_mean, save_invstd, running_mean, running_var, pooled, pooled ? pool_batch * C : 0};
   const int rc = launch_colreduce<0>(x, C, nullptr, M, C, sums_ws, nullptr, nullptr, nullptr, nullptr, 0, nullptr, fin, stream);
   if (rc != TFB_OK) return rc;
@@ -888,12 +883,13 @@ static int bn_apply_launch(const float* x, float* y, int64_t M, int C, const flo
 
 // Training-mode BatchNorm forward from statistics the producing conv / GEMM accumulated in its epilogue: stats = [sum x | sum x^2]
 // (2*C doubles, read only). One launch: no reduction pass over x. pooled (optional): must be ZERO on entry (it is accumulated).
-// Everything else as tfb_bn_fwd.
+// Everything else as tfb_bn_fwd; x, y and residual 16-byte aligned, y16_bf16 8-byte aligned. C <= 2048.
 TFB_API int tfb_bn_fwd_stats(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, float eps, float momentum,
                              int relu, float* running_mean, float* running_var, float* save_mean, float* save_invstd, const double* stats,
                              void* y16_bf16, const float* residual, float* pooled, int pool_batch, cudaStream_t stream) {
   TFB_REQUIRE(x && y && gamma && beta && save_mean && save_invstd && stats && M > 0 && C > 0 && C % 4 == 0 && C <= kBnStatsMaxC);
   TFB_REQUIRE(!pooled || (pool_batch > 0 && M % pool_batch == 0 && !y16_bf16 && !residual));
+  TFB_REQUIRE(aligned16(x) && aligned16(y) && opt16(residual) && opt8(y16_bf16));
   return bn_apply_stats_launch(x, y, M, C, gamma, beta, eps, momentum, relu, running_mean, running_var, save_mean, save_invstd, stats, nullptr,
                                y16_bf16, residual, pooled, pool_batch, stream);
 }
@@ -939,9 +935,12 @@ static int bn_apply_stats_launch(const float* x, float* y, int64_t M, int C, con
 }
 
 // eval-mode BN: normalise with the running statistics (mean, 1/sqrt(var+eps) computed by the caller into save_*).
+// x, y, residual, gamma, beta, mean and invstd 16-byte aligned, y16_bf16 8-byte aligned.
 TFB_API int tfb_bn_apply(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, const float* mean,
                          const float* invstd, int relu, void* y16_bf16, const float* residual, cudaStream_t stream) {
   TFB_REQUIRE(x && y && gamma && beta && mean && invstd && M > 0 && C > 0 && C % 4 == 0);
+  TFB_REQUIRE(aligned16(x) && aligned16(y) && opt16(residual) && opt8(y16_bf16) && aligned16(gamma) && aligned16(beta) && aligned16(mean) &&
+              aligned16(invstd));
   const int64_t total4 = M * C / 4;
   bn_apply_kernel<<<tfb_grid(total4, 256), 256, 0, stream>>>(x, y, total4, C / 4, mean, invstd, gamma, beta, relu,
                                                              (__nv_bfloat16*)y16_bf16, residual);
@@ -986,16 +985,6 @@ static int bn_bwd_impl(const float* x, const float* dy, float* dx, int64_t M, in
                        const float* save_mean, const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws,
                        void* dx16_bf16, const float* ymask, float* gmasked, const float* se_gate, const float* se_dpool, int hw,
                        cudaStream_t stream) {
-  const bool vec = aligned16(x) && aligned16(dy) && aligned16(dx) && (!ymask || aligned16(ymask)) && (!se_gate || (aligned16(se_gate) && aligned16(se_dpool)));
-  if (se_gate && !vec) {
-    // unaligned operands (never the case for the trunks' maps): the squeeze-excite gradient as its own pass (into dx, which the
-    // BatchNorm passes then read as dy and overwrite element by element)
-    const int64_t total = M * C;
-    scale_gate_kernel<<<tfb_grid(total / 4, 256), 256, 0, stream>>>(dy, se_gate, se_dpool, 1.f / (float)hw, dx, total / 4, hw, C);
-    TFB_CHECK_LAUNCH();
-    dy = dx;
-    se_gate = se_dpool = nullptr;
-  }
   const int rc = bn_bwd_reduce(x, dy, M, C, gamma, beta, save_mean, save_invstd, relu, dgamma, dbeta, sums_ws, ymask, se_gate, se_dpool, hw,
                                nullptr, stream);
   if (rc != TFB_OK) return rc;
@@ -1012,11 +1001,14 @@ static int bn_bwd_impl(const float* x, const float* dy, float* dx, int64_t M, in
 // (ymask > 0) with ymask = that y, the masked gradient g = dy * mask drives the BatchNorm backward (pass relu = 0) and is also
 // written to gmasked — it is the gradient of the residual branch.
 // Training-mode BatchNorm backward (timm BatchNormAct2d behind transfuser.py:136-184): dx, dgamma, dbeta (overwritten).
+// x, dy, dx, ymask, gmasked, gamma, beta, save_mean and save_invstd 16-byte aligned, dx16_bf16 8-byte aligned.
 TFB_API int tfb_bn_bwd(const float* x, const float* dy, float* dx, int64_t M, int C, const float* gamma, const float* beta,
                        const float* save_mean, const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws,
                        void* dx16_bf16, const float* ymask, float* gmasked, cudaStream_t stream) {
   TFB_REQUIRE(x && dy && dx && gamma && beta && save_mean && save_invstd && dgamma && dbeta && sums_ws && M > 0 && C > 0 && C % 4 == 0);
   TFB_REQUIRE(!gmasked || ymask);
+  TFB_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx) && opt16(ymask) && opt16(gmasked) && opt8(dx16_bf16) && aligned16(gamma) &&
+              aligned16(beta) && aligned16(save_mean) && aligned16(save_invstd));
   return bn_bwd_impl(x, dy, dx, M, C, gamma, beta, save_mean, save_invstd, relu, dgamma, dbeta, sums_ws, dx16_bf16, ymask, gmasked,
                      nullptr, nullptr, 1, stream);
 }
@@ -1025,12 +1017,15 @@ TFB_API int tfb_bn_bwd(const float* x, const float* dy, float* dx, int64_t M, in
 // reference team_code_transfuser/transfuser.py:136-184 via timm.create_model at :382-384): dy is the gradient of the SE
 // OUTPUT [M = batch * hw, C]; the gradient of the BatchNorm output, dy * se_gate[n][c] + se_dpool[n][c] / hw, is formed inside the
 // two BatchNorm passes (se_gate: the sigmoid gate [batch, C]; se_dpool: gradient of the pooled vector [batch, C], tfb_se_mlp_bwd),
-// replacing tfb_se_bwd_apply (one launch, one write and one read of the map fewer).
+// replacing tfb_se_bwd_apply (one launch, one write and one read of the map fewer). Alignment as for tfb_bn_bwd, and se_gate,
+// se_dpool 16-byte aligned.
 TFB_API int tfb_bn_bwd_se(const float* x, const float* dy, float* dx, int64_t M, int C, const float* gamma, const float* beta,
                           const float* save_mean, const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws,
                           void* dx16_bf16, const float* se_gate, const float* se_dpool, int hw, cudaStream_t stream) {
   TFB_REQUIRE(x && dy && dx && gamma && beta && save_mean && save_invstd && dgamma && dbeta && sums_ws && M > 0 && C > 0 && C % 4 == 0);
   TFB_REQUIRE(se_gate && se_dpool && hw > 0 && M % hw == 0 && M < (int64_t)1 << 31);
+  TFB_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx) && aligned16(se_gate) && aligned16(se_dpool) && opt8(dx16_bf16) && aligned16(gamma) &&
+              aligned16(beta) && aligned16(save_mean) && aligned16(save_invstd));
   return bn_bwd_impl(x, dy, dx, M, C, gamma, beta, save_mean, save_invstd, relu, dgamma, dbeta, sums_ws, dx16_bf16, nullptr, nullptr,
                      se_gate, se_dpool, hw, stream);
 }
@@ -1054,7 +1049,7 @@ TFB_API int tfb_bn_sync_slice(const float* x, int64_t M, int C, const double* st
 // (folded: the sums and the total count N, 2*C + 1 doubles, kept for backward), then normalises with the global mean / biased variance;
 // the running statistics take the unbiased variance over N. from_stats = 0: the normalise pass of tfb_bn_fwd, 1: that of
 // tfb_bn_fwd_stats (with one rank, the same bits as that entry point). pooled (optional): cleared here, then accumulated.
-// Everything else as tfb_bn_fwd.
+// Everything else as tfb_bn_fwd (with from_stats = 1, the alignment of tfb_bn_fwd_stats).
 TFB_API int tfb_bn_fwd_sync(const float* x, float* y, int64_t M, int C, const float* gamma, const float* beta, float eps, float momentum,
                             int relu, float* running_mean, float* running_var, float* save_mean, float* save_invstd, const double* gathered,
                             int world, double* folded, int from_stats, void* y16_bf16, const float* residual, float* pooled, int pool_batch,
@@ -1062,6 +1057,8 @@ TFB_API int tfb_bn_fwd_sync(const float* x, float* y, int64_t M, int C, const fl
   TFB_REQUIRE(x && y && gamma && beta && save_mean && save_invstd && gathered && folded && world > 0 && M > 0 && C > 0 && C % 4 == 0);
   TFB_REQUIRE(!pooled || (pool_batch > 0 && M % pool_batch == 0 && !y16_bf16 && !residual));
   TFB_REQUIRE(!from_stats || C <= kBnStatsMaxC);
+  TFB_REQUIRE(aligned16(x) && aligned16(y) && opt16(residual) && opt8(y16_bf16) &&
+              (from_stats || (aligned16(gamma) && aligned16(beta) && aligned16(save_mean) && aligned16(save_invstd))));
   bn_sync_fold_kernel<<<(C + 255) / 256, 256, 0, stream>>>(gathered, world, C, 1, eps, momentum, save_mean, save_invstd, running_mean,
                                                            running_var, folded, nullptr, pooled, pooled ? pool_batch * C : 0);
   TFB_CHECK_LAUNCH();
@@ -1073,20 +1070,21 @@ TFB_API int tfb_bn_fwd_sync(const float* x, float* y, int64_t M, int C, const fl
 
 // Synchronized BatchNorm backward, step 1 of 2: the reduction pass of tfb_bn_bwd (ymask) / tfb_bn_bwd_se (se_gate, se_dpool, hw),
 // writing this rank's dgamma / dbeta (local, as torch.nn.SyncBatchNorm returns them) and its slice = [sum g | sum g*xhat] (2*C doubles).
-// Operands 16-byte aligned when se_gate is given.
+// x, dy, ymask, se_gate and se_dpool 16-byte aligned.
 TFB_API int tfb_bn_bwd_sync_reduce(const float* x, const float* dy, int64_t M, int C, const float* gamma, const float* beta, const float* save_mean,
                                    const float* save_invstd, int relu, float* dgamma, float* dbeta, double* sums_ws, const float* ymask,
                                    const float* se_gate, const float* se_dpool, int hw, double* slice, cudaStream_t stream) {
   TFB_REQUIRE(x && dy && gamma && beta && save_mean && save_invstd && dgamma && dbeta && sums_ws && slice && M > 0 && C > 0 && C % 4 == 0);
-  TFB_REQUIRE(!se_gate || (se_dpool && hw > 0 && M % hw == 0 && M < (int64_t)1 << 31 && !ymask && aligned16(x) && aligned16(dy) &&
-                           aligned16(se_gate) && aligned16(se_dpool)));
+  TFB_REQUIRE(!se_gate || (se_dpool && hw > 0 && M % hw == 0 && M < (int64_t)1 << 31 && !ymask && aligned16(se_gate) && aligned16(se_dpool)));
+  TFB_REQUIRE(aligned16(x) && aligned16(dy) && opt16(ymask));
   return bn_bwd_reduce(x, dy, M, C, gamma, beta, save_mean, save_invstd, relu, dgamma, dbeta, sums_ws, ymask, se_gate, se_dpool, hw, slice,
                        stream);
 }
 
 // Synchronized BatchNorm backward, step 2 of 2: gathered = the W ranks' slices [W][2*C] in rank order, folded in rank order into
 // gsum (2*C floats of scratch: [sum g | sum g*xhat] over every rank); count = the total row count N of the forward (folded[2*C] of
-// tfb_bn_fwd_sync). dx = gamma * invstd * (g - sum_g/N - xhat * sum_gx/N); dx16_bf16 / ymask / gmasked / se_* as for tfb_bn_bwd(_se).
+// tfb_bn_fwd_sync). dx = gamma * invstd * (g - sum_g/N - xhat * sum_gx/N); dx16_bf16 / ymask / gmasked / se_* as for tfb_bn_bwd(_se),
+// alignment included.
 TFB_API int tfb_bn_bwd_sync_apply(const float* x, const float* dy, float* dx, int64_t M, int C, const float* gamma, const float* beta,
                                   const float* save_mean, const float* save_invstd, int relu, const double* gathered, int world, const double* count,
                                   float* gsum, void* dx16_bf16, const float* ymask, float* gmasked, const float* se_gate, const float* se_dpool,
@@ -1094,6 +1092,8 @@ TFB_API int tfb_bn_bwd_sync_apply(const float* x, const float* dy, float* dx, in
   TFB_REQUIRE(x && dy && dx && gamma && beta && save_mean && save_invstd && gathered && count && gsum && world > 0 && M > 0 && C > 0 &&
               C % 4 == 0);
   TFB_REQUIRE((!gmasked || ymask) && (!se_gate || (se_dpool && hw > 0 && M % hw == 0 && M < (int64_t)1 << 31)));
+  TFB_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx) && opt16(ymask) && opt16(gmasked) && opt16(se_gate) && opt16(se_dpool) &&
+              opt8(dx16_bf16) && aligned16(gamma) && aligned16(beta) && aligned16(save_mean) && aligned16(save_invstd));
   bn_sync_fold_kernel<<<(C + 255) / 256, 256, 0, stream>>>(gathered, world, C, 0, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, gsum,
                                                            nullptr, 0);
   TFB_CHECK_LAUNCH();
