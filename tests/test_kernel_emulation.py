@@ -583,7 +583,8 @@ def test_gpt_up_add_backward_gather(H, W, gh, gw, C):
 
 
 @pytest.mark.parametrize('Hi,Wi,Ho,Wo,C,ac', [(5, 22, 40, 176, 4, 0), (8, 8, 16, 16, 8, 0), (64, 64, 160, 160, 2, 1), (7, 5, 19, 23, 3, 0),
-                                              (7, 5, 19, 23, 3, 1), (6, 6, 6, 6, 4, 1), (9, 9, 4, 5, 4, 0), (4, 4, 1, 1, 4, 1), (2, 3, 40, 50, 3, 0), (2, 3, 40, 50, 3, 1)])
+                                              (7, 5, 19, 23, 3, 1), (6, 6, 6, 6, 4, 1), (9, 9, 4, 5, 4, 0), (4, 4, 1, 1, 4, 1), (2, 3, 40, 50, 3, 0), (2, 3, 40, 50, 3, 1),
+                                              (3, 3, 28, 28, 4, 1)])
 def test_upsample_bilinear_backward_gather(Hi, Wi, Ho, Wo, C, ac):
     """tfb_upsample_bilinear_bwd as a gather (no atomics, no memset): dx written exactly once (NaN-filled destination) and equal to
     autograd through F.interpolate — integer / fractional scales, align_corners on and off, identity and down-sampling sizes."""

@@ -3,9 +3,14 @@
 // the GPT-output "view quirk" + bilinear upsample + add, generic bilinear upsample, dropout, row softmax, bf16 cast.
 // Reference call sites: transfuser.py:129-130 (normalize_imagenet), 150-157 (avgpool, GPT, interpolate, add),
 // 346-364 (token build / output view), 519-522 (softmax, dropout); timm SEModule / Bottleneck add+ReLU.
+#include <assert.h>
+
 #include "common.cuh"
 
 namespace {
+
+// p is a multiple of `bytes` (a null optional operand counts as aligned)
+inline bool tfb_aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
 
 __global__ void __launch_bounds__(256) add_relu_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y,
                                                        int64_t n, int relu, __nv_bfloat16* __restrict__ y16) {
@@ -498,7 +503,8 @@ __device__ __forceinline__ float4 bilinear_adjoint_gather4(const float4* __restr
   int y0, y1, x0, x1;
   lerp_window(gy, gh, H, align_corners, &y0, &y1);
   lerp_window(gx, gw, W, align_corners, &x0, &x1);
-  const int nx = min(x1 - x0 + 1, GATHER_W);           // (callers guarantee windows of at most GATHER_W pixels)
+  const int nx = x1 - x0 + 1;
+  assert(nx <= GATHER_W);                              // tfb_upsample_bilinear_bwd launches this form only for such windows
   float wxs[GATHER_W];
 #pragma unroll
   for (int j = 0; j < GATHER_W; ++j) {
@@ -877,8 +883,10 @@ __global__ void __launch_bounds__(256) se_mlp_bwd2_kernel(const float* __restric
 }  // namespace
 
 // y16_bf16 (optional, here and in tfb_se_scale_fwd): bf16 copy of y written in the same pass.
+// a, b and y 16-byte aligned, y16_bf16 8-byte aligned (four elements per access).
 TFB_API int tfb_add_relu(const float* a, const float* b, float* y, int64_t n, int relu, void* y16_bf16, cudaStream_t stream) {
   TFB_REQUIRE(a && b && y && n >= 0);
+  TFB_REQUIRE(tfb_aligned(a, 16) && tfb_aligned(b, 16) && tfb_aligned(y, 16) && tfb_aligned(y16_bf16, 8));
   if (n == 0) return TFB_OK;
   add_relu_kernel<<<tfb_grid(n / 4 + 1, 256), 256, 0, stream>>>(a, b, y, n, relu, (__nv_bfloat16*)y16_bf16);
   TFB_CHECK_LAUNCH();
@@ -905,9 +913,10 @@ TFB_API int tfb_sigmoid_fwd(const float* x, float* y, int64_t n, cudaStream_t st
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
+// out[n][c] = mean over the HW pixels of x[n][.][c]. C % 4 == 0, x 16-byte aligned.
 TFB_API int tfb_pool_hw_fwd(const float* x, float* out, int N, int HW, int C, cudaStream_t stream) {
   TFB_REQUIRE(x && out && N > 0 && HW > 0 && C > 0);
-  TFB_REQUIRE(C % 4 == 0);
+  TFB_REQUIRE(C % 4 == 0 && tfb_aligned(x, 16));
   if (cudaMemsetAsync(out, 0, (size_t)N * C * sizeof(float), stream) != cudaSuccess) return TFB_ERR_DRIVER;
   int splits = (HW + 255) / 256;
   if (splits > 32) splits = 32;
@@ -926,18 +935,21 @@ TFB_API int tfb_pool_hw_bwd(const float* dout, float* dx, int N, int HW, int C, 
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
+// y[n][p][c] = x[n][p][c] * gate[n][c]. Four channels per access when C % 4 == 0, x, gate and y are 16-byte aligned and y16_bf16
+// 8-byte aligned; one otherwise (the same bits).
 TFB_API int tfb_se_scale_fwd(const float* x, const float* gate, float* y, int N, int HW, int C, void* y16_bf16, cudaStream_t stream) {
   TFB_REQUIRE(x && gate && y && N > 0 && HW > 0 && C > 0);
   const int64_t total = (int64_t)N * HW * C;
   __nv_bfloat16* y16 = (__nv_bfloat16*)y16_bf16;
-  if (C % 4 == 0) scale_nc_kernel<4><<<tfb_grid(total / 4, 256), 256, 0, stream>>>(x, gate, nullptr, 0.f, y, total, HW, C, y16);
+  if (C % 4 == 0 && tfb_aligned(x, 16) && tfb_aligned(gate, 16) && tfb_aligned(y, 16) && tfb_aligned(y16, 8)) scale_nc_kernel<4><<<tfb_grid(total / 4, 256), 256, 0, stream>>>(x, gate, nullptr, 0.f, y, total, HW, C, y16);
   else            scale_nc_kernel<1><<<tfb_grid(total, 256), 256, 0, stream>>>(x, gate, nullptr, 0.f, y, total, HW, C, y16);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
+// dgate[n][c] = sum over the HW pixels of x[n][.][c] * dy[n][.][c]. C % 4 == 0, x and dy 16-byte aligned.
 TFB_API int tfb_se_bwd_reduce(const float* x, const float* dy, float* dgate, int N, int HW, int C, cudaStream_t stream) {
   TFB_REQUIRE(x && dy && dgate && N > 0 && HW > 0 && C > 0);
-  TFB_REQUIRE(C % 4 == 0);
+  TFB_REQUIRE(C % 4 == 0 && tfb_aligned(x, 16) && tfb_aligned(dy, 16));
   if (cudaMemsetAsync(dgate, 0, (size_t)N * C * sizeof(float), stream) != cudaSuccess) return TFB_ERR_DRIVER;
   int splits = (HW + 255) / 256;
   if (splits > 32) splits = 32;
@@ -980,11 +992,13 @@ TFB_API int tfb_se_mlp_bwd(const float* dgate, const float* gate, const float* h
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
+// dx[n][p][c] = dy[n][p][c] * gate[n][c] + dpool[n][c] / HW. Four channels per access when C % 4 == 0 and dy, gate, dpool and dx are
+// 16-byte aligned; one otherwise (the same bits).
 TFB_API int tfb_se_bwd_apply(const float* dy, const float* gate, const float* dpool, float* dx, int N, int HW, int C,
                              cudaStream_t stream) {
   TFB_REQUIRE(dy && gate && dpool && dx && N > 0 && HW > 0 && C > 0);
   const int64_t total = (int64_t)N * HW * C;
-  if (C % 4 == 0) scale_nc_kernel<4><<<tfb_grid(total / 4, 256), 256, 0, stream>>>(dy, gate, dpool, 1.f / (float)HW, dx, total, HW, C, nullptr);
+  if (C % 4 == 0 && tfb_aligned(dy, 16) && tfb_aligned(gate, 16) && tfb_aligned(dpool, 16) && tfb_aligned(dx, 16)) scale_nc_kernel<4><<<tfb_grid(total / 4, 256), 256, 0, stream>>>(dy, gate, dpool, 1.f / (float)HW, dx, total, HW, C, nullptr);
   else            scale_nc_kernel<1><<<tfb_grid(total, 256), 256, 0, stream>>>(dy, gate, dpool, 1.f / (float)HW, dx, total, HW, C, nullptr);
   TFB_CHECK_LAUNCH();
   return TFB_OK;
@@ -1074,8 +1088,10 @@ TFB_API int tfb_upsample_bilinear_fwd(const float* x, float* y, int N, int Hi, i
 TFB_API int tfb_upsample_bilinear_bwd(const float* dy, float* dx, int N, int Hi, int Wi, int Ho, int Wo, int C, int align_corners,
                                       cudaStream_t stream) {
   TFB_REQUIRE(dy && dx && N > 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0 && C > 0);
-  // the float4 form needs every interpolation window to fit the register array of x weights (scale factors up to ~10)
-  const double sx = (double)Wo / (double)Wi;
+  // the float4 form needs every interpolation window to fit the register array of x weights (scale factors up to ~10). A window
+  // spans at most 2 * sx + 5 destination pixels, sx the inverse scale lerp_window divides by: (Wo - 1) / (Wi - 1) with align_corners
+  // (Wo / Wi bounds the whole-row window of Wi == 1 too), Wo / Wi without.
+  const double sx = align_corners && Wi > 1 && Wo > 1 ? (double)(Wo - 1) / (double)(Wi - 1) : (double)Wo / (double)Wi;
   const bool vec = C % 4 == 0 && (int64_t)N * Hi * Wi * C / 4 < 0x7fffffffLL && sx * 2.0 + 5.0 <= (double)GATHER_W &&
                    ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
   if (vec) {
@@ -1091,9 +1107,11 @@ TFB_API int tfb_upsample_bilinear_bwd(const float* dy, float* dx, int N, int Hi,
 // Dropout mask = f(*seed_dev + seed_off, element index): the base seed lives in device memory (advanced by tfb_step_tick once
 // per step, also inside a captured CUDA graph), seed_off identifies the call site; the backward regenerates the same mask.
 // y = dropout(x) (+ residual when given): the mask is a hash of (*seed_dev + seed_off, element index), regenerated in backward.
+// x, y and residual 16-byte aligned (four elements per access).
 TFB_API int tfb_dropout(const float* x, float* y, int64_t n, float p, const uint64_t* seed_dev, uint64_t seed_off, const float* residual,
                         cudaStream_t stream) {
   TFB_REQUIRE(x && y && n >= 0 && p >= 0.f && p < 1.f);
+  TFB_REQUIRE(tfb_aligned(x, 16) && tfb_aligned(y, 16) && tfb_aligned(residual, 16));
   if (n == 0) return TFB_OK;
   dropout_kernel<<<tfb_grid(n / 4 + 1, 256), 256, 0, stream>>>(x, y, n, p, seed_dev, seed_off, residual);
   TFB_CHECK_LAUNCH();
@@ -1113,8 +1131,10 @@ TFB_API int tfb_softmax_bwd(const float* P, const float* dPd, float* dS, int64_t
   TFB_CHECK_LAUNCH();
   return TFB_OK;
 }
+// y = bf16(x). x 16-byte aligned, y 8-byte aligned (four elements per access).
 TFB_API int tfb_cast_bf16(const float* x, void* y, int64_t n, cudaStream_t stream) {
   TFB_REQUIRE(x && y && n >= 0);
+  TFB_REQUIRE(tfb_aligned(x, 16) && tfb_aligned(y, 8));
   if (n == 0) return TFB_OK;
   cast_bf16_kernel<<<tfb_grid(n / 4 + 1, 256), 256, 0, stream>>>(x, (__nv_bfloat16*)y, n);
   TFB_CHECK_LAUNCH();
