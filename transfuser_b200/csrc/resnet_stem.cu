@@ -214,6 +214,9 @@ maxpool3s2_bwd_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ 
   }
 }
 
+// p is a multiple of `bytes` (a null optional operand counts as aligned)
+inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 }  // namespace
 
 TFB_API int tfb_conv7x7s2_fwd(const float* x, const float* w, float* y, int N, int H, int W, int Cin, int Cout, cudaStream_t stream) {
@@ -238,8 +241,10 @@ TFB_API int tfb_conv7x7s2_wgrad(const float* x, const float* dy, float* dw, int 
   }
 }
 
+// C % 4 == 0; x and y 16-byte aligned, argmax_u8 4-byte aligned, y16_bf16 8-byte aligned (four channels per access).
 TFB_API int tfb_maxpool3x3s2_fwd(const float* x, float* y, void* y16_bf16, void* argmax_u8, int N, int H, int W, int C, cudaStream_t stream) {
   TFB_REQUIRE(x && y && argmax_u8 && N > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0);
+  TFB_REQUIRE(aligned(x, 16) && aligned(y, 16) && aligned(argmax_u8, 4) && aligned(y16_bf16, 8));
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   maxpool3s2_fwd_kernel<<<tfb_grid((int64_t)N * Ho * Wo * (C / 4), 256), 256, 0, stream>>>(
       x, y, static_cast<__nv_bfloat16*>(y16_bf16), static_cast<uint8_t*>(argmax_u8), N, H, W, C, Ho, Wo);
@@ -247,8 +252,10 @@ TFB_API int tfb_maxpool3x3s2_fwd(const float* x, float* y, void* y16_bf16, void*
   return TFB_OK;
 }
 
+// C % 4 == 0; dy and dx 16-byte aligned, argmax_u8 4-byte aligned (four channels per access).
 TFB_API int tfb_maxpool3x3s2_bwd(const float* dy, const void* argmax_u8, float* dx, int N, int H, int W, int C, cudaStream_t stream) {
   TFB_REQUIRE(dy && argmax_u8 && dx && N > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0);
+  TFB_REQUIRE(aligned(dy, 16) && aligned(dx, 16) && aligned(argmax_u8, 4));
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   maxpool3s2_bwd_kernel<<<tfb_grid((int64_t)N * H * W * (C / 4), 256), 256, 0, stream>>>(
       dy, static_cast<const uint8_t*>(argmax_u8), dx, N, H, W, C, Ho, Wo);
